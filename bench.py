@@ -1,6 +1,6 @@
 """bench.py — decode tokens/sec of the soft-attention LSTM decode path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl sat|reference] [--workload 2|3]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl sat|reference] [--workload 2|3|4|5] [--dump-outputs DIR]
     (N > 1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...)
 
 A "step" is one pass of the hot path over one batch of synthetic contexts: project the
@@ -16,6 +16,8 @@ batches larger than L2.  Weights: random U(-0.08, 0.08) of the reference archite
   cpu_baseline  the numpy oracle (oracle/ref_step.py, "port": TensorFlow cannot be installed
             here) on the host cores, bounded sample
 --impl reference times that CPU restatement as its own arm (rank 0 only).
+--dump-outputs DIR writes what the last timed step returned (see dump_outputs) so that two builds can be compared
+output for output: inputs and weights are seeded, identical from run to run.
 """
 import argparse
 import json
@@ -37,7 +39,7 @@ WORKLOADS = {
     # BASELINE.json configs[3]: training step, 64 images per GPU (512 on 8 GPUs), forward + backward + gradient
     # all-reduce + clip + Adam; tokens = teacher-forced words per step
     4: dict(name="config4: training step B=64/GPU L=196 D=512 H=1024 V=10000 T=20, fwd+bwd+all-reduce+Adam (large "
-                 "products on the tcgen05 dense kernel as split bf16x3, the rest fp32 CUDA-core kernels; dropout on)", B=64, L=196, D=512, H=1024, V=10000, T=20, train=True),
+                 "products on the wgmma dense kernel as split bf16x3, the rest fp32 CUDA-core kernels; dropout on)", B=64, L=196, D=512, H=1024, V=10000, T=20, train=True),
     # BASELINE.json configs[4]: beam search, 128 images x beam 3, T=30 (tokens = images x T)
     5: dict(name="config5: beam search beam=3, 128 images, L=196 D=512 H=1024 V=10000 T=30 (device-side TopN)",
             B=128, L=196, D=512, H=1024, V=10000, T=30, beam=3),
@@ -49,7 +51,31 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+    # NVIDIA's data sheet for the H100 SXM (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet")
+
+
+DUMP_MAX_ELEMS = 1 << 21      # per array: larger outputs are replaced by a fixed, seeded sample of this many elements
+
+
+def dump_outputs(out_dir, arrays):
+    """Write every array as out_dir/<name>.npy: integer arrays as float64 (exact), the rest as float32.  An array with
+    more than DUMP_MAX_ELEMS elements is stored as the sample x.ravel()[idx], idx = the sorted first DUMP_MAX_ELEMS of a
+    permutation drawn from numpy's RandomState(0): the same elements in every run, at most 16 MB per array."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, x in arrays.items():
+        if hasattr(x, "detach"):
+            x = x.detach().cpu().numpy()
+        x = np.asarray(x)
+        x = x.astype(np.float64 if x.dtype.kind in "iub" else np.float32)
+        if x.size > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.RandomState(0).permutation(x.size)[:DUMP_MAX_ELEMS])
+            x = x.ravel()[idx]
+        total += x.nbytes
+        assert total <= 64 << 20, "dumped outputs exceed 64 MB"
+        np.save(os.path.join(out_dir, name + ".npy"), x)
 
 
 class ClockSampler(threading.Thread):
@@ -222,8 +248,8 @@ def bench_config(wl, world, pool=None, pool_mb=None):
                 "the prologue of batch i+1 runs under the decode steps of batch i" % (T, B))
     return {"workload": wl["name"], "per_gpu_batch": B, "global_batch": B * world,
             "parallelism": "dp%d (batch sharded, replicated weights, no data-path collective in decoding)" % world,
-            "precision": "fp32 in/out; GEMMs as split bf16x3 on tcgen05 with fp32 TMEM accumulation",
-            "l2": ("inputs rotate over %d context batches (%.0f MB + 137 MB weights/activations) > 126 MB L2" % (pool, pool_mb))
+            "precision": "fp32 in/out; GEMMs as split bf16x3 on wgmma with fp32 register accumulation",
+            "l2": ("inputs rotate over %d context batches (%.0f MB + 137 MB weights/activations) > 50 MB L2" % (pool, pool_mb))
                   if pool else "inputs larger than L2 (context batches rotate)",
             "step": step}
 
@@ -246,9 +272,10 @@ def run_reference(args, wl, rank, world):
     print(json.dumps(line), flush=True)
 
 
-def measure_training(wl, model, rank, local_rank, world, dev, steps, warmup, e2e=True, sample_clocks=True):
+def measure_training(wl, model, rank, local_rank, world, dev, steps, warmup, e2e=True, sample_clocks=True, dump=None):
     """config 4: one optimisation step per bench step (forward + backward + gradient all-reduce + clip + Adam); weak
-    scaling, 64 images per GPU.  Returns the record (rank 0) or None."""
+    scaling, 64 images per GPU.  Returns the record (rank 0) or None.  dump: directory for the last timed step's
+    losses, squared gradient norm and updated parameters (dump_outputs)."""
     import torch
     import torch.distributed as dist
     from sat_b200 import parallel
@@ -280,9 +307,11 @@ def measure_training(wl, model, rank, local_rank, world, dev, steps, warmup, e2e
     with torch.cuda.stream(st):
         ev0.record(st)
         for i in range(steps):
-            model.train_step(ctx_dev[i % pool], sent, masks, seed=100 + i, sync=False)   # losses stay on the device
+            last = model.train_step(ctx_dev[i % pool], sent, masks, seed=100 + i, sync=False)   # losses stay on the device
         ev1.record(st)
     barrier()
+    if dump and rank == 0:
+        dump_outputs(dump, {"losses": last[0], "grad_sq_norm": last[1], "params": model.params})
     ms = parallel.max_over_ranks(ev0.elapsed_time(ev1), dev)
     clocks = sampler.stop() if (rank == 0 and sample_clocks) else None
     value = world * B * T * steps / (ms / 1e3)
@@ -331,7 +360,7 @@ def measure_training(wl, model, rank, local_rank, world, dev, steps, warmup, e2e
 
 def run_training(args, wl, model, cfg, rank, local_rank, world, dev):
     import torch.distributed as dist
-    rec = measure_training(wl, model, rank, local_rank, world, dev, args.steps, args.warmup)
+    rec = measure_training(wl, model, rank, local_rank, world, dev, args.steps, args.warmup, dump=args.dump_outputs)
     if rank == 0:
         line = {"metric": rec["metric"], "value": rec["value"], "unit": "tokens/s", "n_gpus": world, "steps": args.steps,
                 "warmup": rec["warmup"], "ms_per_step": rec["ms_per_step"], "higher_is_better": True, "scaling": "weak",
@@ -356,8 +385,10 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the CPU baseline leg")
     ap.add_argument("--no-train", action="store_true", help="skip the training sub-record of the default line")
     ap.add_argument("--pool", type=int, default=6, help="distinct context batches rotated through")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (see dump_outputs)")
     ap.add_argument("--profile-run", action="store_true",
-                    help="for runs under ncu: only the device-resident timed loop (no clock pre/post roll, no e2e, no roofline legs)")
+                    help="for runs under a profiler: only the device-resident timed loop (no clock pre/post roll, no e2e, no roofline legs)")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     rank = int(os.environ.get("RANK", "0"))
@@ -374,7 +405,7 @@ def main():
     from sat_b200 import parallel
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: no CUDA device visible (there is no CPU fallback)")
+        raise SystemExit("bench.py needs an H100: no CUDA device visible (there is no CPU fallback)")
     torch.cuda.set_device(local_rank)
     if world > 1:
         parallel.init_process_group("nccl")
@@ -416,8 +447,8 @@ def main():
 
     def loop(i):
         if beam > 1:
-            return model.beam_device(ctx_dev[i % pool], beam, T, 2)[0]
-        return model.loop_device(ctx_dev[i % pool], T)[0]
+            return model.beam_device(ctx_dev[i % pool], beam, T, 2)
+        return model.loop_device(ctx_dev[i % pool], T)
 
     for i in range(max(args.warmup, 3) + 2 * pool):       # warm-up also builds one CUDA graph per pool entry
         loop(i)
@@ -444,10 +475,13 @@ def main():
     with torch.cuda.stream(st):
         ev0.record(st)
         for i in range(args.steps):
-            loop(i)
+            last = loop(i)
         ev1.record(st)
     barrier()
     ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        names = ("sentences", "lengths", "scores", "num_results", "completed") if beam > 1 else ("tokens", "logits")
+        dump_outputs(args.dump_outputs, {n: x for n, x in zip(names, last) if x is not None})
     launches = model.info("launches")
     if not args.profile_run:
         roll(0.3, len(sampler.rows) + 2 if rank == 0 else 0)
@@ -563,7 +597,7 @@ def main():
             return (both - base) / reps
         loop_grid = model.info("att_loop_grid")       # CTAs of the attention launches inside the timed decode loop
         att_ns_full = time_attention(0)                # whole GPU
-        att_ns = time_attention(loop_grid) if 0 < loop_grid < 148 else att_ns_full
+        att_ns = time_attention(loop_grid) if 0 < loop_grid < model.info("num_sms") else att_ns_full
         # per-family times of one eager step (cold L2), for the breakdown
         model.set_option("profile", 1)
         lw = torch.zeros(B, dtype=torch.int32, device=dev)
@@ -578,14 +612,8 @@ def main():
         model.set_option("profile", 0)
         att_bytes = 4 * (B * L * (D + A) + B * A + A + B * L + B * D)       # SURVEY.md §8(d)
         achieved = att_bytes / att_ns                                       # bytes/ns == GB/s
-        # DRAM traffic is NOT measured by this run (it needs ncu): the figure below is read from the committed ncu capture
-        # and labelled as such
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "att_traffic.json")   # dram__bytes_read+write of one ncu --set full capture
-        if os.path.exists(tp) and args.workload == 2:
-            tj = json.load(open(tp))
-            traffic = tj["dram_bytes_read"] + tj["dram_bytes_write"]
-            traffic_src = "not measured in this run: " + tj["source"]
+        # DRAM traffic is not measured by this run (it needs a hardware-counter profiler)
+        traffic, traffic_src = None, "not measured"
         roof = dict(bound="hbm", achieved=achieved, peak=pk["hbm"], unit="GB/s", frac=achieved / pk["hbm"],
                     traffic=traffic, traffic_source=traffic_src,
                     kernel=("att_wpc_kernel<1>" if (D == 512 and A == 512) else "att_fused_kernel<1>"),

@@ -1,5 +1,5 @@
 /* sat_b200.h — C ABI of libsat_b200.so: the soft-attention LSTM decode path of
- * Cheng-Lin-Li/show-attend-and-tell on NVIDIA B200 (sm_100a).
+ * Cheng-Lin-Li/show-attend-and-tell on NVIDIA H100 (sm_90a).
  *
  * The reference has no FFI: its boundary is the Python attribute surface of
  * CaptionGenerator consumed through tf.Session.run feeds/fetches.  Each entry point
@@ -66,11 +66,11 @@ int sat_version(void);
 
 /* integer knobs (defaults in brackets; all of them are for experiments and tests, none changes results beyond
  * the summation order noted):
- *   "gemm"        1 = tcgen05 [1], 0 = CUDA-core bring-up kernels
+ *   "gemm"        1 = wgmma tensor cores [1], 0 = CUDA-core bring-up kernels
  *   "umma_layout" 0 = interleaved [0], 1 = 128B swizzle; must be set before sat_set_weight
  *   "graphs"      1 = replay CUDA graphs in loops [1]
  *   "hoist"       1 = project the contexts once per image batch [1]; 0 = recompute every step like model.py:259-262
- *   "pa"          1 = activations travel between dense layers as packed UMMA operands [1]
+ *   "pa"          1 = activations travel between dense layers as packed MMA operands [1]
  *   "xpack"       1 = cooperative activation pre-pass when operands are not packed [1]; 0 = producer warps
  *   "pdl"         1 = launches carry the programmatic-dependent-launch attribute [1]
  *   "overlap"     launch layout of the greedy loop: 2 = one stream, the attention kernel of step t+1 runs beside the
@@ -90,7 +90,7 @@ int sat_version(void);
  *   "profile"     1 = record CUDA events around every eager kernel launch; read back with sat_get_info
  *                 "prof_ns_<family>" / "prof_n_<family>"
  *   "trace"       1 / 2 / 3 = in-kernel globaltimer stamps of a dense launch ("trace_at") / of the attention kernel /
- *                 of every launch of a loop (tools/trace*.py, tools/timeline.py)
+ *                 of every launch of a loop
  * Environment: SAT_PDL=0 creates handles with "pdl" off (for tools that expect one kernel of a stream at a time).
  * A handle expects the GPU to itself while a loop runs: the fused arg-max of the vocabulary layer ends in a grid-wide
  * rendezvous of its one-wave launch (a stuck rendezvous traps with a message after a few seconds). */
@@ -183,7 +183,7 @@ int sat_dense_fwd(sat_handle* h, const float* x, const float* w_tf, const float*
  *     sat_train_forward_backward  ->  all-reduce(sum) of `grads` across ranks (NCCL)  ->  sat_train_apply
  * Dropout masks come from a counter-based generator keyed by `seed` (0 = dropout off), so a step is
  * reproducible; ranks must use different seeds.
- * Knobs: sat_set_option "train_tc" 1 = the large products of the step run on the tcgen05 dense kernel [1], 0 = fp32
+ * Knobs: sat_set_option "train_tc" 1 = the large products of the step run on the wgmma dense kernel [1], 0 = fp32
  * CUDA-core SGEMM everywhere.  Environment switches, read once per process, for A/B timing (results agree to round-off):
  * SAT_TRAIN_PDL=0 launches the step's kernels without the programmatic-serialization attribute; SAT_TRAIN_DEC_ALL=0 keeps
  * the decode layers inside the time loop (default: one stacked product per layer for all T steps); SAT_TRAIN_SIDE=0 keeps

@@ -1,4 +1,4 @@
-"""Build libsat_b200.so in-tree with nvcc for sm_100a (no GPU needed: nvcc cross-compiles).
+"""Build libsat_b200.so in-tree with nvcc for sm_90a (no GPU needed: nvcc cross-compiles).
 
     python show-attend-and-tell_b200/build.py [--force] [--verbose]
 
@@ -17,7 +17,7 @@ OUT = os.path.join(HERE, "libsat_b200.so")
 STAMP = os.path.join(HERE, "build", "stamp.txt")
 SOURCES = ["sat_api.cu", "sat_linear.cu", "sat_chain.cu", "sat_attention.cu", "sat_rows.cu", "sat_train.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3", "--expt-relaxed-constexpr",
 ]
 
@@ -68,7 +68,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(out)
     if failed:
         raise RuntimeError("nvcc compilation failed")
-    link = [nvcc, "-shared", "-o", OUT, *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+    link = [nvcc, "-shared", "-o", OUT, *objs, "-gencode", "arch=compute_90a,code=sm_90a",
             "-Xcompiler", "-fPIC", "-cudart", "static", "-Xlinker", "--exclude-libs,ALL"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:

@@ -147,7 +147,7 @@ struct sat_handle {
     unsigned* chain_ctr = nullptr;         // [kChainMaxPhase + kChainMaxPhase * kChainMaxTiles]
     float* chain_scratch = nullptr;
     unsigned long long* chain_best = nullptr;
-    int opt_chain = 0, opt_chain_cluster = 0;   // (measured slower than the per-layer launches so far: opt-in, see DESIGN.md)
+    int opt_chain = 0, opt_chain_cluster = 0;   // (opt-in: see fused_loop_available)
     int chain_clusters[9] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};   // resident clusters of the chained kernel per cluster size
     const unsigned* att_qflag = nullptr;   // set around the attention launch that runs beside a chained launch
     unsigned att_qtarget = 0;
@@ -291,14 +291,15 @@ extern "C" int sat_create(const sat_dims* dims, sat_handle** out) {
     h->d = d;
     // SAT_PDL=0: start with programmatic dependent launch off (option "pdl").  For tools that assume one kernel of a
     // stream at a time: compute-sanitizer's synccheck reports warps of an early-started kernel as divergent at their
-    // first block barrier (profiles/r02_sanitizer_synccheck.log).
+    // first block barrier.
     if (const char* e = getenv("SAT_PDL")) h->opt_pdl = (e[0] == '0') ? 0 : 1;
     int rc = SAT_OK;
     auto body = [&]() -> int {
         CK(cudaGetDevice(&h->dev));
         cudaDeviceProp prop;
         CK(cudaGetDeviceProperties(&prop, h->dev));
-        if (prop.major != 10) return fail(SAT_ERR_UNSUPPORTED, "device sm_%d%d is not sm_100", prop.major, prop.minor);
+        if (prop.major != 9 || prop.minor != 0)   // (the library holds sm_90a code only)
+            return fail(SAT_ERR_UNSUPPORTED, "device sm_%d%d is not sm_90", prop.major, prop.minor);
         h->num_sms = prop.multiProcessorCount;
         CK(cudaDeviceGetAttribute(&h->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->dev));
         CK(lin_init_attrs());
@@ -579,7 +580,7 @@ static LinSeg seg(const float* p, int ld, int width, const int32_t* gather = nul
 }
 
 static int row_tile_for(int rows) {
-    const int nrt = (rows + 255) / 256;
+    const int nrt = (rows + kMaxRowTile - 1) / kMaxRowTile;
     const int per = (rows + nrt - 1) / nrt;
     return ((per + 15) / 16) * 16;
 }
@@ -604,9 +605,8 @@ static int plan(sat_handle* h, Layer& ly, LinProblem& P, std::initializer_list<L
     P.K = ly.K;
     P.k_blocks = ly.k_blocks;
     P.rows = rows;
-    P.n_row_tiles = (rows + 255) / 256;
-    int per = (rows + P.n_row_tiles - 1) / P.n_row_tiles;
-    P.row_tile = ((per + 15) / 16) * 16;
+    P.row_tile = row_tile_for(rows);
+    P.n_row_tiles = (rows + P.row_tile - 1) / P.row_tile;
     P.n_out = ly.n_out;
     P.n_tiles = ly.n_tiles;
     P.wpack = ly.wpack;
@@ -701,7 +701,7 @@ static int launch(sat_handle* h, LinProblem* probs, int n, cudaStream_t st) {
     return SAT_OK;
 }
 
-// Dense product on the tcgen05 kernel from operands that are ALREADY in the packed layouts (training path,
+// Dense product on the wgmma kernel from operands that are ALREADY in the packed layouts (training path,
 // sat_train.cu): out[rows, n_out] (+)= X * W with X a packed activation of row tile `row_tile` and W a packed weight.
 int sat_handle_layout_mode(sat_handle* h) { return h->opt_layout; }
 int sat_handle_train_tc(sat_handle* h) { return h->opt_train_tc && h->opt_gemm != 0; }
@@ -710,7 +710,7 @@ int sat_dense_packed(sat_handle* h, const uint8_t* x_pa, int rows, int row_tile,
                      const float* bias_packed, int n_out, int epi, float* out, int ldo, int accumulate, int splits,
                      void* stream, int weights_dynamic) {
     if (!h || !x_pa || !wpack || !out) return fail(SAT_ERR_INVALID, "sat_dense_packed: null argument");
-    if (K % kBK || row_tile % 16 || row_tile > 256 || splits < 1 || splits > 8 || (splits & (splits - 1)))
+    if (K % kBK || row_tile % 16 || row_tile > kMaxRowTile || splits < 1 || splits > 8 || (splits & (splits - 1)))
         return fail(SAT_ERR_INVALID, "sat_dense_packed: K %d / row tile %d / splits %d", K, row_tile, splits);
     LinProblem P;
     memset(&P, 0, sizeof(P));
@@ -1287,9 +1287,8 @@ static int loop_enqueue_chain(sat_handle* h, const float* ctx, int B, int T, con
 //   chain(t) = { LSTM(t) -> [decode fc_1(t) || q(t+1)] -> vocabulary layer(t) + arg-max }  ->  attention(t+1)
 // The attention kernel of step t+1 starts beside the chained launch, spins on the counter of its phase 1 (q(t+1) and
 // everything older are complete then) and runs beside the vocabulary phase on the SMs whose CTAs have exited.
-// OPT-IN (option "chain" = 1; default 0): measured SLOWER than the per-layer launches at config 2 (50 us against 38 us per
-// step: its three epilogues and the last arriver's tail run from cold instruction caches and cost 7 - 9 us each, see
-// DESIGN.md), and only validated for a 64-row tile (at B = 4 an eager, fully serialised run of it was seen to give wrong
+// OPT-IN (option "chain" = 1; default 0): its three epilogues and the last arriver's tail run from cold instruction
+// caches, which made it slower than the per-layer launches where it was timed; and only validated for a 64-row tile (at B = 4 an eager, fully serialised run of it was seen to give wrong
 // logits from the second step on while the replayed graph was right: unresolved, so smaller batches are refused).
 static bool fused_loop_available(sat_handle* h, int B) {
     return h->opt_chain && h->pa_ok && h->opt_pa && h->opt_gemm != 0 && h->opt_overlap == 2 && h->opt_pdl &&
@@ -1450,13 +1449,20 @@ static int loop_enqueue_fused(sat_handle* h, const float* ctx, int B, int T, con
     return SAT_OK;
 }
 
+// The overlapped and chained loops hand the chosen word on inside the vocabulary layer: they need its fused arg-max,
+// i.e. every CTA of that layer resident in one wave.
+static bool vocab_argmax_fits(sat_handle* h, int B) {
+    return h->dec_2.n_tiles * ((B + kMaxRowTile - 1) / kMaxRowTile) <= h->num_sms;
+}
+
 static int loop_enqueue(sat_handle* h, const float* ctx, int B, int T, const int32_t* forced, int32_t* tokens,
                         float* logits_all, cudaStream_t st) {
     const bool pa = h->pa_ok && h->opt_pa && h->opt_gemm != 0;
+    const bool am = pa && vocab_argmax_fits(h, B);
     if (fused_loop_available(h, B)) return loop_enqueue_fused(h, ctx, B, T, forced, tokens, logits_all, st, false);
-    if (pa && h->opt_overlap == 2 && h->opt_pdl && h->d.num_decode_layers == 2)
+    if (am && h->opt_overlap == 2 && h->opt_pdl && h->d.num_decode_layers == 2)
         return loop_enqueue_chain(h, ctx, B, T, forced, tokens, logits_all, st);
-    if (pa && h->opt_overlap && h->d.num_decode_layers == 2 && st != nullptr && st != cudaStreamLegacy)
+    if (am && h->opt_overlap && h->d.num_decode_layers == 2 && st != nullptr && st != cudaStreamLegacy)
         return loop_enqueue_overlap(h, ctx, B, T, forced, tokens, logits_all, st);
     RET(prepare_impl(h, ctx, B, h->st_c[0], h->st_h[0], st, pa ? h->pa_h[0] : nullptr));
     CK(cudaMemsetAsync(h->word, 0, (size_t)B * sizeof(int32_t), st));  // <start> = 0 (model.py:254)
@@ -1482,9 +1488,9 @@ static int loop_enqueue(sat_handle* h, const float* ctx, int B, int T, const int
     return SAT_OK;
 }
 
-static bool chain_loop_available(sat_handle* h) {
+static bool chain_loop_available(sat_handle* h, int B) {
     return h->pa_ok && h->opt_pa && h->opt_gemm != 0 && h->opt_overlap == 2 && h->opt_pdl && h->d.num_decode_layers == 2 &&
-           h->opt_hoist && h->d.num_attend_layers == 2;
+           h->opt_hoist && h->d.num_attend_layers == 2 && vocab_argmax_fits(h, B);
 }
 
 // Greedy / teacher-forced loop with its prologue on a second stream (option "xbatch", and always for the pipelined
@@ -1555,7 +1561,7 @@ extern "C" int sat_decode_loop(sat_handle* h, const float* contexts, int32_t B, 
     if (B < 1 || B > h->max_rows) return fail(SAT_ERR_INVALID, "batch %d outside [1, %d]", B, h->max_rows);
     if (T < 1) return fail(SAT_ERR_INVALID, "T must be >= 1");
     cudaStream_t st = (cudaStream_t)stream;
-    if (h->opt_xbatch && chain_loop_available(h) && st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread)
+    if (h->opt_xbatch && chain_loop_available(h, B) && st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread)
         return decode_loop_xbatch(h, contexts, B, T, forced_words, tokens, logits_all, st, nullptr);
     std::vector<long long> key = {1, (long long)contexts, B, T, (long long)forced_words, (long long)tokens,
                                   (long long)logits_all};
@@ -1744,7 +1750,7 @@ extern "C" int sat_decode_loop_host_submit(sat_handle* h, const float* contexts_
     if (forced) CK(cudaMemcpyAsync(forced, forced_words_host, TB * sizeof(int32_t), cudaMemcpyHostToDevice, h->pipe_copy));
     CK(cudaEventRecord(h->pipe_up[slot], h->pipe_copy));
     CK(cudaStreamWaitEvent(st, h->pipe_up[slot], 0));      // (forced words; and the contexts when not overlapped)
-    if (chain_loop_available(h) && st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread)
+    if (chain_loop_available(h, B) && st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread)
         RET(decode_loop_xbatch(h, h->pipe_ctx[slot], B, T, forced, tok, nullptr, st, h->pipe_up[slot]));
     else
         RET(sat_decode_loop(h, h->pipe_ctx[slot], B, T, forced, tok, nullptr, stream));

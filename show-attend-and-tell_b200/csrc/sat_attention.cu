@@ -61,7 +61,7 @@ __device__ __forceinline__ void att_pack_embedding(const AttParams& p, int first
             ll[i] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
         }
         const int rt = b / p.pa_row_tile, r = b - rt * p.pa_row_tile;
-        uint8_t* dst = p.emb_pa + ((size_t)rt * (p.emb_E >> 6) + (gi >> 3)) * 2 * half + umma_tile_off(p.pa_mode, r, gi & 7);
+        uint8_t* dst = p.emb_pa + ((size_t)rt * (p.emb_E >> 6) + (gi >> 3)) * 2 * half + mma_tile_off(p.pa_mode, r, gi & 7);
         *reinterpret_cast<uint4*>(dst) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
         *reinterpret_cast<uint4*>(dst + half) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
     }

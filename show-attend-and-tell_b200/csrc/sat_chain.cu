@@ -6,34 +6,34 @@
 //
 // Why one launch.  Each layer needs the complete output of the layer before it, and every layer alone is one CTA per SM
 // (its pipeline stages fill the shared memory), so with one launch per layer a successor CTA becomes resident only when
-// the predecessor CTA on its SM has EXITED — after its tail — and then starts its weight stream cold.  In-loop traces of
-// the per-layer launches (profiles/r01_kernel_timelines.txt, profiles/r02_loop_dram_traffic.csv) show the weights ~75 %
-// L2 resident and the step nevertheless at 45 us: cold starts, tails and dependency releases, not bandwidth.  Here
+// the predecessor CTA on its SM has EXITED — after its tail — and then starts its weight stream cold: with the weights
+// largely L2 resident, cold starts, tails and dependency releases rather than bandwidth bound such a step.  Here
 // every CTA is resident for the whole step; its TMA lane keeps streaming the (immutable) weights of its NEXT tile into
 // the stages the tensor core has released, i.e. under the epilogue and the rendezvous of the current phase, and the
 // phases meet at grid-wide arrival counters (one L2 round trip) instead of at kernel boundaries.
 //
-// Same arithmetic as lin_umma_kernel (sat_linear.cu): swap-AB tcgen05 tiles (128 outputs x row_tile batch rows), packed
-// bf16 hi/lo operands fetched by 1-D bulk TMA, three MMAs per K step, fp32 accumulation in TMEM, split-K partials summed
-// in fixed split order — the two kernels produce bit-identical results.  Differences: split-K partials meet in an L2
+// Same arithmetic as lin_mma_kernel (sat_linear.cu): swap-AB wgmma tiles (128 outputs x row_tile batch rows), packed
+// bf16 hi/lo operands fetched by 1-D bulk TMA, three MMAs per K step, fp32 accumulation in registers, split-K partials
+// summed in fixed split order — the two kernels produce bit-identical results.  Differences: split-K partials meet in an L2
 // resident scratch buffer behind a per-tile arrival counter (no thread-block clusters: the grid need not be cut into
 // clusters and phases may use different split factors); the accumulator tile is parked in a shared-memory region of its
 // own (the stages belong to the next tile's weights by then); the arg-max of the vocabulary phase is one atomicMax per
 // (row, tile) on the ordered 64-bit key, all CTAs but the last to arrive exit at once, and the last arriver records
 // the words and packs their embedding rows for the next step.
 //
-// Warp roles (384 threads): warp 0 = weight TMA warp (runs ahead across phases), warp 10 = activation TMA warp (a phase's
-// activations only after the counter of the phase before says they are complete), warps 1 and 11 = MMA issue (even / odd
-// K blocks, two TMEM accumulators; warp 1 also owns the TMEM allocation), warps 2-9 = epilogues.
+// Warp roles (320 threads): warps 0-7 = two warpgroups that issue the wgmma (accumulator in registers) and run the
+// epilogues, warp 8 = weight TMA warp (runs ahead across phases), warp 9 = activation TMA warp (a phase's activations
+// only after the counter of the phase before says they are complete).
 #include "sat_common.cuh"
 #include "sat_linear.cuh"
 #include "sat_linear_dev.cuh"
 
 namespace sat {
 
-constexpr int kChainThreads = kLinThreads + 64;   // + warp 10: the activation TMA warp, warp 11: the second MMA warp
-constexpr int kChainXWarp = kLinThreads / 32;
-constexpr int kChainMma2Warp = kChainXWarp + 1;
+constexpr int kChainThreads = kLinThreads;
+constexpr int kChainWWarp = kLinProducers / 32;   // warp 8
+constexpr int kChainXWarp = kChainWWarp + 1;      // warp 9
+constexpr int kChainNT = 4;                       // accumulator fragments: row tile 64, the only one the loop uses
 
 struct ChainJob {
     const LinProblem* P;
@@ -52,7 +52,7 @@ __device__ __forceinline__ void chain_job(const LinChain& C, int ph, ChainJob& J
     J.P = &P;
     J.split = local % P.splits;
     J.n_tile = local / P.splits;
-    J.kb0 = (P.k_blocks * J.split) / P.splits;               // (same rounding as lin_umma_kernel's 64-bit form)
+    J.kb0 = (P.k_blocks * J.split) / P.splits;               // (same rounding as lin_mma_kernel's 64-bit form)
     J.nkb = (P.k_blocks * (J.split + 1)) / P.splits - J.kb0;
     J.tile_id = (pi ? F.p[0].n_tiles : 0) + J.n_tile;
     J.cta0 = (int)blockIdx.x - J.split;
@@ -63,11 +63,9 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
     uint64_t* full_w = reinterpret_cast<uint64_t*>(smem_raw);  // [stages]
     uint64_t* full_x = full_w + 8;
     uint64_t* empty = full_x + 8;
-    uint64_t* tmem_full = empty + 8;
-    uint64_t* gather_bar = tmem_full + 1;                        // embedding rows of the last arriver's tail
+    uint64_t* gather_bar = empty + 8;                            // embedding rows of the last arriver's tail
     uint64_t* peer_ready = gather_bar + 1;                       // [kChainMaxPhase] every split of my tile has parked its partial
     uint64_t* peer_done = peer_ready + kChainMaxPhase;           // [kChainMaxPhase] every split of my tile has read mine
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(peer_done + kChainMaxPhase);
     unsigned* flag_s = reinterpret_cast<unsigned*>(smem_raw + 256);
     int* word_s = reinterpret_cast<int*>(smem_raw + 512);      // [<= 64] words picked by the last arriver
     uint8_t* stage_base = smem_raw + 1024;
@@ -78,9 +76,6 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
     const uint32_t x_stage_bytes = 2 * x_half_bytes;
     const uint32_t stage_bytes = kWStageBytes + x_stage_bytes;
     float* tile_s = reinterpret_cast<float*>(stage_base + (size_t)S * stage_bytes);   // [N][128] fp32, own region
-    uint32_t acc_stride = 32;                  // TMEM columns per accumulator; two of them (even / odd K blocks)
-    while ((int)acc_stride < N) acc_stride <<= 1;
-    const uint32_t tmem_cols = 2 * acc_stride;
 
     ChainJob job[kChainMaxPhase];
 #pragma unroll
@@ -89,7 +84,6 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
     unsigned long long* const dbg1 = (C.dbg_mode == 1 || C.dbg_mode == 2) ? C.dbg : nullptr;   // per-K-block stamps of phase 0
     unsigned long long* const dbg3 = C.dbg_mode == 3 ? C.dbg : nullptr;   // fine stamps of K blocks 0..3 of phase 0
     unsigned long long* const dbg4 = C.dbg_mode == 4 ? C.dbg : nullptr;   // epilogue internals: phase 0 (6..12), last arriver's tail (0..5)
-    const bool hi_only = C.dbg_mode == 2;   // timing experiment only (WRONG results): one MMA per K step instead of three
 
     if (threadIdx.x == 0) {
         trace_stamp(dbg0, 0);
@@ -97,9 +91,8 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
         for (int s = 0; s < S; ++s) {
             mbar_init(&full_w[s], 1);
             mbar_init(&full_x[s], 1);
-            mbar_init(&empty[s], 1);
+            mbar_init(&empty[s], kLinProducers / 32);   // one arrival per consumer warp once its MMAs are complete
         }
-        mbar_init(tmem_full, 2);                // one arrival per MMA warp and tile
         mbar_init(gather_bar, 1);
 #pragma unroll
         for (int ph = 0; ph < kChainMaxPhase; ++ph) {            // (used once each: one tile per phase and launch)
@@ -109,20 +102,13 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
         }
         fence_mbar_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_ptr, tmem_cols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
     // (cluster mode: a peer may arrive on this CTA's peer_ready / peer_done barriers as soon as it runs: they must be
     // initialised cluster-wide first.  All threads, once, before anything waits for the predecessor launch.)
     if (C.cluster > 1) cluster_sync_all();
-    const uint32_t tmem_d = *tmem_ptr;
 
-    if (warp == 0 || warp == kChainXWarp) {
-        // ===================== TMA warps: warp 0 streams the weights, warp 10 the activations =====================
+    if (warp == kChainWWarp || warp == kChainXWarp) {
+        // ===================== TMA warps: warp 8 streams the weights, warp 9 the activations =====================
         // The K blocks of this CTA's tiles form one sequence over the phases.  A block's weight half is issued as soon
         // as its stage is free (weights are immutable: no dependency, so this warp runs ahead into the next phase's
         // tile under the epilogue and the rendezvous of the current one); its activation half is issued by the other
@@ -130,7 +116,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
         // whole tile, so: two warps (the wait -> arm -> issue chains of the two halves overlap), each converged with one
         // elected lane issuing (see elect_one), every decision a warp vote, everything needed a running cursor in
         // registers — no divisions, no indexed reads of the launch descriptor.
-        const bool wside = warp == 0;
+        const bool wside = warp == kChainWWarp;
         const uint64_t wpol = l2_policy(C.l2_w);
         const int l2w = wside ? C.l2_w : 0;
         const uint32_t stage0 = smem_u32(stage_base) + (wside ? 0u : (uint32_t)kWStageBytes);
@@ -197,7 +183,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
             }
             ready_ph = 0;                          // activations of phases <= ready_ph may be fetched
         }
-        // (no busy polling: these warps share their schedulers with the epilogue warps, and a spinning warp takes issue
+        // (no busy polling: these warps share their schedulers with the consumer warps, and a spinning warp takes issue
         // slots from them — the stage wait suspends in hardware (mbarrier.try_wait), the phase wait sleeps between polls)
         while (ph < kChainMaxPhase) {
             if (ph > ready_ph) {
@@ -208,8 +194,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
                     if ((++spins & 1023) == 0) {
                         if (spins == 1024) t0 = clock64();
                         else if (clock64() - t0 > SAT_SPIN_LIMIT_CYCLES) {
-                            if (lane == 0) printf("sat_b200: chained dense launch: phase %d never completed (block %d)\n", ph - 1, (int)blockIdx.x);
-                            __trap();
+                            __trap();   // the phase before never completed
                         }
                     }
                 }
@@ -217,87 +202,16 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
                 ready_ph = ph;
                 if (C.tl && lane == 0) tl_begin(C.tl + 4 * (1 + ph));   // (timeline) first CTA that saw the phase open
             }
-            mbar_wait(&empty[st], par);
+            mbar_wait_mma(&empty[st], par);
             issue();
         }
-    } else if (warp == 1 || warp == kChainMma2Warp) {
-        // ===================== MMA warps: warp 1 takes the even K blocks of a tile, warp 11 the odd ones =====================
-        // At 64 batch rows an MMA is short (128 x 64 x 16: ~48 cycles, bound by reading its 6 KB of operands from shared
-        // memory) and the issuing thread is held for about as long per instruction, so ONE warp's wait -> 12 MMAs ->
-        // commit chain leaves the tensor core idle between K blocks (0.57 us per block measured against 0.3 us of MMAs).
-        // Two warps alternate blocks into two accumulators (TMEM columns [0, N) and [acc_stride, acc_stride + N), summed
-        // when the epilogue reads them): one warp's waits and commits run under the other's MMAs.  Converged warps: all
-        // lanes wait on the stage barriers, one elected lane issues (see elect_one).
-        {
-            const int odd = warp == 1 ? 0 : 1;
-            const uint32_t idesc = umma_idesc_bf16(kTileN, N);
-            const uint32_t lbo = mode == 0 ? 128u : 16u;
-            const uint32_t layout = mode == 0 ? 0u : 2u;
-            const uint32_t kstep16 = (mode == 0 ? 256u : 32u) >> 4;   // descriptor address units (16 B) per UMMA K step
-            // descriptor of the byte address 0 of this operand class; the start address field (>> 4) is added per use
-            const uint64_t dzero = umma_smem_desc(0u, lbo, 1024, layout);
-            const uint32_t stage0 = smem_u32(stage_base);
-            const uint32_t tmem_acc = __shfl_sync(0xffffffffu, tmem_d, 0) + (odd ? acc_stride : 0u);
-            int s = 0;
-            uint32_t par = 0u;
-#pragma unroll
-            for (int ph = 0; ph < kChainMaxPhase; ++ph) {
-                const int nkb = job[ph].nkb;
-                if (nkb == 0) continue;
-                // (the accumulators are free: the activations of this tile only exist once this CTA's previous epilogue
-                // has arrived at its phase counter, i.e. after it has read the accumulators out)
-#pragma unroll 1
-                for (int it = 0; it < nkb; ++it) {
-                    if ((it & 1) == odd) {
-                        mbar_wait(&full_w[s], par);
-                        if (dbg3 && ph == 0 && it < 4 && lane == 0) trace_stamp(dbg3, 12 + it);
-                        mbar_wait(&full_x[s], par);
-                        if (lane == 0) {
-                            if (dbg3 && ph == 0 && it < 4) trace_stamp(dbg3, 4 + it);
-                            if (dbg0 && it == 0) trace_stamp(dbg0, ph == 0 ? 2 : ph == 1 ? 9 : 11);      // first operands of the phase landed
-                            if (dbg1 && ph == 0 && it < 8) trace_stamp(dbg1, it);
-                        }
-                        tc_fence_after();
-                        if (elect_one()) {
-                            // (14-bit start-address field: in a cluster launch a shared-memory address carries the
-                            // CTA's rank in its high bits, which must not leak into the descriptor's other fields)
-                            const uint32_t wb = stage0 + (uint32_t)s * stage_bytes;
-                            uint64_t a_hi = dzero + (uint64_t)((wb >> 4) & 0x3FFFu);
-                            uint64_t a_lo = dzero + (uint64_t)(((wb + kWHalfBytes) >> 4) & 0x3FFFu);
-                            uint64_t b_hi = dzero + (uint64_t)(((wb + kWStageBytes) >> 4) & 0x3FFFu);
-                            uint64_t b_lo = dzero + (uint64_t)(((wb + kWStageBytes + x_half_bytes) >> 4) & 0x3FFFu);
-#pragma unroll
-                            for (int kk = 0; kk < kBK / 16; ++kk) {
-                                umma_f16(tmem_acc, a_hi, b_hi, idesc, (it >= 2 || kk != 0) ? 1u : 0u);   // first own block starts the sum
-                                if (!hi_only) {
-                                    umma_f16(tmem_acc, a_lo, b_hi, idesc, 1u);
-                                    umma_f16(tmem_acc, a_hi, b_lo, idesc, 1u);
-                                }
-                                a_hi += kstep16; a_lo += kstep16; b_hi += kstep16; b_lo += kstep16;
-                            }
-                            umma_commit(&empty[s]);
-                            if (dbg3 && ph == 0 && it < 4) trace_stamp(dbg3, 8 + it);
-                        }
-                        __syncwarp();
-                    }
-                    if (++s == S) { s = 0; par ^= 1u; }
-                }
-                // this warp's part of the tile is issued: arrive at tmem_full when its MMAs are complete (a warp with
-                // no block of a one-block tile arrives at once)
-                if (elect_one()) {
-                    if (nkb > odd) umma_commit(tmem_full);
-                    else mbar_arrive(tmem_full);
-                    if (dbg0 && ph == 0 && !odd) trace_stamp(dbg0, 3);
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp < kChainXWarp) {
-        // ===================== epilogues (warps 2..9) =====================
-        const int pt = threadIdx.x - 64;   // 0..255
+    } else if (warp < kChainWWarp) {
+        // ===================== consumer warpgroups (warps 0..7): MMA, epilogues =====================
+        const int pt = threadIdx.x;   // 0..255
         const int u = pt & 31;
         if (C.pdl) { pdl_wait(); pdl_launch_dependents(); }
-        int jc = 0;                        // tiles finished by this CTA: parity of tmem_full
+        int s = 0;                         // pipeline stage of the next K block (one sequence over the phases)
+        uint32_t par = 0u;
         int wait_done_ph = -1;             // cluster mode: phase whose peer_done barrier guards tile_s
 #pragma unroll 1
         for (int ph = 0; ph < C.nphase; ++ph) {
@@ -326,7 +240,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
             const bool row_loop = epi == kEpiLstm || out != nullptr || out_pa != nullptr;
             float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
             if (epi != kEpiNone && P.bias) bias4 = *reinterpret_cast<const float4*>(P.bias + n_tile * kTileN + 4 * u);
-            const float bias_fold = (do_am && P.bias) ? P.bias[n_tile * kTileN + (warp & 3) * 32 + lane] : 0.f;
+            const float* const bias_fold = (do_am && P.bias) ? P.bias + n_tile * kTileN : nullptr;
             float cpre[2] = {0.f, 0.f};
             if (epi == kEpiLstm && unit < Hh) {
 #pragma unroll
@@ -335,38 +249,35 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
                     if (idx < hi) cpre[j] = c_in[(size_t)(idx >> 5) * Hh + unit];
                 }
             }
-            // ---- part 1: accumulator TMEM -> shared memory (and, split-K, the rows other CTAs reduce -> L2 scratch)
+            // ---- main loop: per K block, both warpgroups issue their 64 x N x 64 share of the three products
+            AccTile<kChainNT> acc;
+#pragma unroll 1
+            for (int it = 0; it < j_nkb; ++it) {
+                mbar_wait_mma(&full_w[s], par);
+                if (dbg3 && ph == 0 && it < 4 && pt == 0) trace_stamp(dbg3, 12 + it);
+                mbar_wait_mma(&full_x[s], par);
+                if (pt == 0) {
+                    if (dbg3 && ph == 0 && it < 4) trace_stamp(dbg3, 4 + it);
+                    if (dbg0 && it == 0) trace_stamp(dbg0, ph == 0 ? 2 : ph == 1 ? 9 : 11);      // first operands of the phase landed
+                    if (dbg1 && ph == 0 && it < 8) trace_stamp(dbg1, it);
+                }
+                mma_kblock(acc, smem_u32(stage_base) + (uint32_t)s * stage_bytes, x_half_bytes, mode, it == 0);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);   // frees the stage: this warp's MMAs have read it
+                if (++s == S) { s = 0; par ^= 1u; }
+            }
+            // ---- part 1: accumulator -> shared memory (and, split-K, the rows other CTAs reduce -> L2 scratch)
             {
-                const int q = warp & 3;               // TMEM lane quadrant this warp may access
-                const int half = (warp - 2) >> 2;     // 0 or 1
-                const int nl = q * 32 + lane;         // output feature within the tile (TMEM lane)
-                mbar_wait(tmem_full, (uint32_t)jc & 1u);
-                tc_fence_after();
                 if (C.tl && pt == 0) { tl_main_done(C.tl); tl_go(C.tl + 4 * (1 + ph)); tl_main_done(C.tl + 4 * (1 + ph)); }
                 if (dbg0 && pt == 0) trace_stamp(dbg0, ph == 0 ? 4 : ph == 1 ? 10 : 12);
                 if (dbg4 && pt == 0 && ph == 0) trace_stamp(dbg4, 6);
-                const uint32_t taddr = tmem_d + ((uint32_t)(q * 32) << 16);
                 float* const my_part = C.scratch + (size_t)blockIdx.x * N * kTileN;
                 // (cluster mode: the peers of my PREVIOUS split tile must have finished reading tile_s before it is rewritten)
                 if (wait_done_ph >= 0) { mbar_wait_cluster(&peer_done[wait_done_ph], 0u); wait_done_ph = -1; }
-#pragma unroll 1
-                for (int c0 = half * 16; c0 < N; c0 += 32) {
-                    float v[16];
-                    tmem_ld16(taddr + (uint32_t)c0, v);
-                    if (j_nkb > 1) {                       // + the odd K blocks' accumulator
-                        float v2[16];
-                        tmem_ld16(taddr + acc_stride + (uint32_t)c0, v2);
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) v[j] += v2[j];
-                    }
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int row = c0 + j;
-                        tile_s[row * kTileN + nl] = v[j] + bias_fold;
-                        if (gsplit && row < rows_here && (row * 32 < lo || row * 32 >= hi)) __stcg(my_part + row * kTileN + nl, v[j]);
-                    }
-                }
-                tc_fence_before();
+                acc_for_each(acc, N, [&](int m, int row, float v) {
+                    tile_s[row * kTileN + m] = bias_fold ? v + bias_fold[m] : v;
+                    if (gsplit && row < rows_here && (row * 32 < lo || row * 32 >= hi)) __stcg(my_part + row * kTileN + m, v);
+                });
                 if (dbg4 && pt == 0 && ph == 0) trace_stamp(dbg4, 7);
             }
             const uint32_t tile_addr = smem_u32(tile_s);
@@ -392,7 +303,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
                 if (pt == 0) {
                     unsigned* tc = C.tile_ctr + ph * kChainMaxTiles + j_tile_id;
                     atomicAdd(tc, 1u);
-                    wait_counter(tc, C.tile_target[ph], "split-K rendezvous of a chained dense launch");
+                    wait_counter_mma(tc, C.tile_target[ph]);   // split-K rendezvous
                     __threadfence();
                     if (ph == 0) trace_stamp(dbg0, 6);
                     if (ph == 0) trace_stamp(dbg4, 9);
@@ -443,7 +354,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
                                           : idx == idx0 ? (r < 4 ? pfa[r & 3] : pfb[r & 3])
                                           : (idx == idx1 && pre1) ? pfb[r & 3]
                                                                   : remote(r, bb);
-                        g = part[0];   // fixed split order: bit-identical to the cluster reduction of lin_umma_kernel
+                        g = part[0];   // fixed split order: bit-identical to the cluster reduction of lin_mma_kernel
 #pragma unroll
                         for (int r = 1; r < 8; ++r)
                             if (r < splits) { g.x += part[r].x; g.y += part[r].y; g.z += part[r].z; g.w += part[r].w; }
@@ -571,7 +482,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
                                 if (elect_one())
                                     tma_bulk_g2s(stage_base + (size_t)r * row_pitch, P.am_emb + (size_t)word_s[r] * E, row_bytes, gather_bar);
                             if (dbg4 && pt == 0) trace_stamp(dbg4, 2);
-                            mbar_wait(gather_bar, 0);
+                            mbar_wait_mma(gather_bar, 0);
                             if (dbg4 && pt == 0) trace_stamp(dbg4, 3);
                         }
                         // conversion fp32 -> packed bf16 hi / lo.  Task t = one 16-byte group of the destination; the low
@@ -608,7 +519,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
                                 if (rs[j] < rows) {
                                     uint4 hi4, lo4;
                                     split_bf16x8(a4[j], c4[j], hi4, lo4);
-                                    uint8_t* dst = P.am_emb_pa + (size_t)kbs[j] * 2 * halfb + umma_tile_off(mode, rs[j], kg);
+                                    uint8_t* dst = P.am_emb_pa + (size_t)kbs[j] * 2 * halfb + mma_tile_off(mode, rs[j], kg);
                                     *reinterpret_cast<uint4*>(dst) = hi4;
                                     *reinterpret_cast<uint4*>(dst + halfb) = lo4;
                                 }
@@ -618,18 +529,12 @@ __global__ void __launch_bounds__(kChainThreads, 1) lin_chain_kernel(const __gri
                 }
             }
             if (dbg4 && pt == 0 && do_am && flag_s[0]) trace_stamp(dbg4, 4);
-            ++jc;
         }
         // (cluster mode: a CTA's shared memory must outlive the peers' reads of it)
         if (wait_done_ph >= 0) mbar_wait_cluster(&peer_done[wait_done_ph], 0u);
     }
     __syncthreads();
     if (threadIdx.x == 0) { trace_stamp(dbg0, 5); trace_stamp(dbg4, 5); tl_end(C.tl); }
-    if (warp == 1) {
-        __syncwarp();
-        tc_fence_after();
-        tmem_dealloc(tmem_d, tmem_cols);
-    }
 }
 
 // ------------------------------------------------------------ host side
@@ -673,7 +578,7 @@ int lin_chain_max_clusters(int row_tile, int stages, int cluster) {
 }
 
 cudaError_t lin_chain_launch(const LinChain& C, int grid, cudaStream_t st) {
-    if (C.stages < 2 || C.row_tile > 64 || C.row_tile % 16) return cudaErrorInvalidValue;
+    if (C.stages < 2 || C.row_tile != 16 * kChainNT) return cudaErrorInvalidValue;   // (the MMA width is the row tile)
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(kChainThreads);

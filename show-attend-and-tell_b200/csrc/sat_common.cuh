@@ -1,6 +1,6 @@
-// sat_common.cuh — sm_100a PTX wrappers shared by the sat_b200 kernels:
-// mbarrier, TMA (cp.async.bulk / cp.async.bulk.tensor), tcgen05 (TMEM alloc,
-// UMMA issue, commit, TMEM load), proxy fences.  Hand-written inline PTX; no
+// sat_common.cuh — sm_90a PTX wrappers shared by the sat_b200 kernels:
+// mbarrier, TMA (cp.async.bulk / cp.async.bulk.tensor), wgmma (warpgroup MMA
+// from shared-memory descriptors), proxy fences.  Hand-written inline PTX; no
 // CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda_runtime.h>
@@ -10,7 +10,7 @@
 
 #ifndef SAT_SPIN_LIMIT_CYCLES
 // A barrier wait that lasts longer than this many SM cycles (~4 s) is a bug:
-// trap instead of hanging the GPU box.
+// trap instead of hanging the GPU.
 #define SAT_SPIN_LIMIT_CYCLES (8000000000ll)
 #endif
 
@@ -68,6 +68,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         }
     }
 }
+// Kernels that issue wgmma (sat_linear.cu, sat_chain.cu) use the _mma forms of the waits: no printf, because a call
+// (vprintf) anywhere in such a kernel makes ptxas serialise its MMAs (C7510).  A hang there ends in a bare trap.
+__device__ __forceinline__ void mbar_wait_mma(uint64_t* bar, uint32_t parity) {
+    if (mbar_try_wait(bar, parity)) return;
+    const long long t0 = clock64();
+    while (!mbar_try_wait(bar, parity))
+        if (clock64() - t0 > SAT_SPIN_LIMIT_CYCLES) __trap();
+}
 
 // ----------------------------------------------------------------------- TMA
 // 1-D bulk copy global -> shared, completion on an mbarrier (UBLKCP).
@@ -84,7 +92,7 @@ __device__ __forceinline__ void prefetch_l2_bulk(const void* src_gmem, uint32_t 
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src_gmem), "r"(bytes) : "memory");
 }
 // L2 eviction-priority policies for TMA loads: 0 = none, 1 = evict_first (streamed once per step),
-// 2 = evict_last (weights: keep resident in the 126 MB L2 across decode steps), 3 = evict_normal.
+// 2 = evict_last (weights: keep resident in the 50 MB L2 across decode steps), 3 = evict_normal.
 __device__ __forceinline__ uint64_t l2_policy(int kind) {
     uint64_t pol = 0;
     if (kind == 1) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
@@ -130,7 +138,7 @@ __device__ __forceinline__ void tma_tensor2d_g2s_hint(void* dst_smem, const void
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (TMA / UMMA reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -140,10 +148,9 @@ __device__ __forceinline__ void fence_proxy_async_global() {
     asm volatile("fence.proxy.async.global;" ::: "memory");
 }
 
-// One lane of a CONVERGED warp (elect.sync).  The async-unit instructions (cp.async.bulk, tcgen05.mma / commit) take their
+// One lane of a CONVERGED warp (elect.sync).  The async-unit instructions (cp.async.bulk) take their
 // operands from the uniform register file: issued from `if (lane == 0)` code their addresses live in per-thread registers
-// and every instruction costs a handful of register->uniform moves plus an elect/branch loop (~70 cycles per MMA measured
-// on the chained dense launch); issued as `if (elect_one()) ...` from a loop the whole warp runs, the operands are
+// and every instruction costs a handful of register->uniform moves plus an elect/branch loop; issued as `if (elect_one()) ...` from a loop the whole warp runs, the operands are
 // computed in uniform registers to begin with.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
@@ -151,70 +158,131 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
-// ------------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// --------------------------------------------------------------------- wgmma
+// Warpgroup MMA: the four warps of an aligned warpgroup issue together, the accumulator lives in their registers.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16 inputs / fp32 accumulate.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// All previously issued UMMAs of this thread arrive on `bar` when complete
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// TMEM -> registers: 32 lanes x 32 bit, 16 consecutive columns per thread.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// d[64 x N] (+)= A[64 x 16] * B[N x 16]^T for N = 16, 32, ..., 128: bf16 inputs from shared-memory descriptors, both
+// K-major, fp32 accumulate; scale_d == 0: d = A * B (the previous contents are ignored), else d += A * B.
+// Fragment of thread t of the warpgroup (w = t / 32, l = t % 32): d[4i + 2h + e] is row w*16 + l/4 + 8h, column
+// 8i + 2(l%4) + e.
+template <int N>
+struct Wgmma;
+
+template <>
+struct Wgmma<16> {
+    static __device__ __forceinline__ void mma(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(desc_a), "l"(desc_b), "r"(scale_d)
+            : "memory");
+    }
+};
+
+template <>
+struct Wgmma<32> {
+    static __device__ __forceinline__ void mma(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(desc_a), "l"(desc_b), "r"(scale_d)
+            : "memory");
+    }
+};
+
+template <>
+struct Wgmma<48> {
+    static __device__ __forceinline__ void mma(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "l"(desc_a), "l"(desc_b), "r"(scale_d)
+            : "memory");
+    }
+};
+
+template <>
+struct Wgmma<64> {
+    static __device__ __forceinline__ void mma(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(desc_a), "l"(desc_b), "r"(scale_d)
+            : "memory");
+    }
+};
+
+template <>
+struct Wgmma<80> {
+    static __device__ __forceinline__ void mma(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39}, %40, %41, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+            : "l"(desc_a), "l"(desc_b), "r"(scale_d)
+            : "memory");
+    }
+};
+
+template <>
+struct Wgmma<96> {
+    static __device__ __forceinline__ void mma(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, %48, %49, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+            : "l"(desc_a), "l"(desc_b), "r"(scale_d)
+            : "memory");
+    }
+};
+
+template <>
+struct Wgmma<112> {
+    static __device__ __forceinline__ void mma(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n112k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55}, %56, %57, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+            : "l"(desc_a), "l"(desc_b), "r"(scale_d)
+            : "memory");
+    }
+};
+
+template <>
+struct Wgmma<128> {
+    static __device__ __forceinline__ void mma(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(desc_a), "l"(desc_b), "r"(scale_d)
+            : "memory");
+    }
+};
+// pins the n accumulator registers at this point of the instruction stream (no access is moved across it)
+__device__ __forceinline__ void wgmma_fence_operand(float* d, int n) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < n; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor (sm_100 format, version field = 1).
+// Shared-memory matrix descriptor of wgmma (sm_90 format).
 //   bits [0,14)  start address >> 4      bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4 bits [46,48) version = 1
-//   bits [61,64) layout: 0 = no swizzle (interleave), 2 = 128B swizzle
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
+//   bits [32,46) stride byte offset >> 4 bits [62,64) layout: 0 = no swizzle (interleave), 1 = 128B swizzle
+__device__ __forceinline__ uint64_t gmma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
                                                    uint32_t layout) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)(layout & 7) << 61;
+    d |= (uint64_t)(layout & 3) << 62;
     return d;
-}
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32, both operands K-major.
-//   [4,6) c_format=1 (F32)  [7,10) a_format=1 (BF16)  [10,13) b_format=1 (BF16)
-//   bit 15 a_major=0 (K)  bit 16 b_major=0 (K)  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ __forceinline__ uint32_t umma_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 // ------------------------------------------------ programmatic dependent launch
@@ -275,10 +343,7 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
         if (ok) return;
         if ((++spins & 255) == 0) {
             if (spins == 256) t0 = clock64();
-            else if (clock64() - t0 > SAT_SPIN_LIMIT_CYCLES) {
-                printf("sat_b200: cluster mbarrier wait timed out (block %d thread %d)\n", (int)blockIdx.x, (int)threadIdx.x);
-                __trap();
-            }
+            else if (clock64() - t0 > SAT_SPIN_LIMIT_CYCLES) __trap();   // cluster mbarrier wait (wgmma kernels only)
         }
     }
 }
@@ -334,7 +399,7 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// spin until a monotonic arrival counter has reached `target` (wrap-safe); traps instead of hanging the GPU box
+// spin until a monotonic arrival counter has reached `target` (wrap-safe); traps instead of hanging the GPU
 __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p);
 __device__ __forceinline__ void wait_counter(const unsigned* ctr, unsigned target, const char* what) {
     if ((int)(ld_acquire_gpu(ctr) - target) >= 0) return;
@@ -345,6 +410,11 @@ __device__ __forceinline__ void wait_counter(const unsigned* ctr, unsigned targe
             __trap();
         }
     }
+}
+__device__ __forceinline__ void wait_counter_mma(const unsigned* ctr, unsigned target) {   // (see mbar_wait_mma)
+    const long long t0 = clock64();
+    while ((int)(ld_acquire_gpu(ctr) - target) < 0)
+        if (clock64() - t0 > SAT_SPIN_LIMIT_CYCLES) __trap();
 }
 __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
     unsigned v;

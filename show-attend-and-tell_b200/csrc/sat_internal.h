@@ -7,7 +7,7 @@ const sat_dims* sat_handle_dims(sat_handle* h);
 void** sat_handle_train_slot(sat_handle* h);
 void sat_handle_set_train_free(sat_handle* h, void (*fn)(void*));
 
-// dense product on the tcgen05 kernel from packed operands (see sat_api.cu); epi = sat::kEpi* of sat_linear.cuh.
+// dense product on the wgmma kernel from packed operands (see sat_api.cu); epi = sat::kEpi* of sat_linear.cuh.
 // weights_dynamic: the packed weight was produced by the kernel launched just before (it must not be prefetched
 // ahead of the dependency wait).
 int sat_dense_packed(sat_handle* h, const uint8_t* x_pa, int rows, int row_tile, int K, const uint8_t* wpack,

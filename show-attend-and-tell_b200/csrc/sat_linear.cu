@@ -1,4 +1,4 @@
-// sat_linear.cu — small-batch dense layers on tcgen05 tensor cores.
+// sat_linear.cu — small-batch dense layers on Hopper tensor cores (wgmma).
 //
 // Computes, for up to 4 grouped problems per launch,
 //     out[b, n] = epilogue( sum_k X[b, k] * W[k, n] + bias[n] )
@@ -6,14 +6,14 @@
 // (model.py:276-279) of the reference.  The batch is small (4..384) and the
 // weights are large, so every problem is bound by streaming W once from HBM.
 //
-// Formulation ("swap-AB"): the weight matrix is the UMMA M operand — a CTA owns
-// 128 output features x a K-range — and the batch rows are the UMMA N operand
+// Formulation ("swap-AB"): the weight matrix is the MMA M operand — a CTA owns
+// 128 output features x a K-range — and the batch rows are the MMA N operand
 // (16..256).  fp32 parity (1e-3 vs the fp32 reference) is kept with a
 // split-precision product: W and X are each held as bf16 hi + bf16 lo
 // (w = hi + lo to 16 mantissa bits) and three MMAs are issued per K-step,
-//     acc += Whi*Xhi + Wlo*Xhi + Whi*Xlo        (fp32 accumulation in TMEM).
+//     acc += Whi*Xhi + Wlo*Xhi + Whi*Xlo        (fp32 accumulation in registers).
 // W is repacked once at sat_set_weight() into the exact shared-memory image of
-// the UMMA K-major operand (hi and lo halves adjacent: 4 bytes per weight, the
+// the wgmma K-major operand (hi and lo halves adjacent: 4 bytes per weight, the
 // same HBM traffic as the fp32 original), so a pipeline stage is filled by ONE
 // 32 KB cp.async.bulk (TMA) per CTA.  X (tiny) arrives the same way when its
 // producer kernel wrote it as a "packed activation" (x_mode 2, the steady state
@@ -26,14 +26,15 @@
 // (bit-reproducible), then the fused epilogue runs (bias / tanh / LSTM gates /
 // greedy argmax of the vocabulary layer / packed copy for the next layer).
 //
-// Warp roles (320 threads): warp 0 = TMA producer (one lane), warp 1 = TMEM
-// allocator + MMA issuer (one lane), warps 2..9 = X producers (modes 0/1), then
-// epilogue.
+// Warp roles (320 threads): warps 0..7 = two warpgroups that issue the wgmma
+// (warpgroup g: outputs [64g, 64g + 64) of the tile, accumulator in registers),
+// convert X (modes 0/1) and run the epilogue; warp 8 = TMA producer (one lane),
+// warp 9 = activation TMA stream (x_mode 2).
 //
 // Launch chaining: every launch carries the programmatic-dependent-launch attribute.  The TMA lane fills its
 // first stages with weights before griddepcontrol.wait; launch_dependents is called only after the wait (so a
-// kernel never starts before the predecessor of its predecessor has completed).  While the main loop streams,
-// the idle epilogue warps run the (short) epilogue once without side effects to pull its code into the
+// kernel never starts before the predecessor of its predecessor has completed).  While the first stages are in
+// flight, the consumer warps run the (short) epilogue once without side effects to pull its code into the
 // instruction caches: epilogues execute once per launch from cold caches, and that costs microseconds.
 // The vocabulary layer's fused arg-max ends in a grid-wide rendezvous of its one-wave launch; CTA i then merges
 // row i's candidates and packs the embedding row of the chosen word for the next LSTM / decode layers.
@@ -79,19 +80,19 @@ __device__ __forceinline__ float epi_scalar(const LinProblem& P, float acc, int 
     return P.epi == kEpiBiasTanh ? act_tanh(acc) : acc;
 }
 
-// ------------------------------------------------------------- UMMA kernel
+// ------------------------------------------------------------- wgmma kernel
 struct XChunk {
     float4 a[2], c[2];
 };
 
-__global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_constant__ LinLaunch L) {
+// NT = (row tile of the launch) / 16: the accumulator fragments per warpgroup
+template <int NT>
+__global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_constant__ LinLaunch L) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // control block: barriers etc. live in the first 1024 bytes
     uint64_t* full_w = reinterpret_cast<uint64_t*>(smem_raw);  // [stages]
     uint64_t* full_x = full_w + 8;
     uint64_t* empty = full_x + 8;
-    uint64_t* tmem_full = empty + 8;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
     uint8_t* stage_base = smem_raw + 1024;
     const bool xpa = L.x_mode == 2;   // every X segment was packed by its producer kernel
     const bool xpre = L.x_mode == 1;  // activations packed by a cooperative pre-pass of this launch
@@ -119,8 +120,8 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
     const int mode = L.layout_mode;
     const uint32_t x_half_bytes = (uint32_t)N * kBK * 2;
     const uint32_t stage_bytes = kWStageBytes + 2 * x_half_bytes;
-    uint32_t tmem_cols = 32;
-    while ((int)tmem_cols < N) tmem_cols <<= 1;
+    constexpr int kTmaWarp = kLinProducers / 32;   // warp 8
+    constexpr int kXWarp = kTmaWarp + 1;           // warp 9
 
     // ---- one-time setup
     if (threadIdx.x == 0) {
@@ -128,23 +129,15 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
         tl_begin(L.tl);
         for (int s = 0; s < S; ++s) {
             mbar_init(&full_w[s], 1);
-            mbar_init(&full_x[s], xtma ? 1 : kLinProducers);
-            mbar_init(&empty[s], 1);
+            mbar_init(&full_x[s], 1);
+            mbar_init(&empty[s], kLinProducers / 32);   // one arrival per consumer warp once its MMAs are complete
         }
-        mbar_init(tmem_full, 1);
         fence_mbar_init();
-    }
-    if (warp == 1) {
-        tmem_alloc(tmem_ptr, tmem_cols);
-        tmem_relinquish();
     }
     // grid-barrier generation must be sampled before this CTA can possibly arrive on it
     unsigned gen0 = 0;
-    if (xpre && threadIdx.x == 0) gen0 = ld_acquire_gpu(P.xbar + 1);
-    tc_fence_before();
+    if (xpre && threadIdx.x == kTmaWarp * 32) gen0 = ld_acquire_gpu(P.xbar + 1);
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_d = *tmem_ptr;
     const uint32_t x_stage_bytes = 2 * x_half_bytes;
     float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);   // epilogue warps: bias of this thread's 4 outputs
     // Programmatic dependent launch: everything above touched no global memory.  The weights are immutable
@@ -152,14 +145,13 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
     // global access (activations, outputs) waits for the predecessor.
     // launch_dependents is issued only AFTER the wait, which gives every kernel of the chain the invariant
     // "when I start, everything before my immediate predecessor is complete and visible".
-    // Only the epilogue warps (and, later, the TMA lane) wait: the MMA lane touches no global memory, and a
-    // blocking wait issued by the idle lanes of warp 0 would stall the TMA lane's weight prefetch with them.
-    if (L.pdl && warp >= 2) { pdl_wait(); pdl_launch_dependents(); }
+    // Every warp but the TMA warp waits here (the TMA lane waits later): a blocking wait issued by the idle lanes of
+    // the TMA warp would stall the TMA lane's weight prefetch with them.
+    if (L.pdl && warp != kTmaWarp) { pdl_wait(); pdl_launch_dependents(); }
 
     // ---- TMA production when every operand arrives packed (x_mode 2: the steady state of loops and of the training
-    // step's products).  Two warps: warp 0 streams the weight halves of the stages (immutable: it starts before the
-    // dependency wait), the last epilogue warp streams the activation halves before it joins the epilogue — the two
-    // wait -> arm -> issue chains overlap, and this production paces the tile.  Each is a WHOLE warp running the loop
+    // step's products).  Two warps: warp 8 streams the weight halves of the stages (immutable: it starts before the
+    // dependency wait), warp 9 streams the activation halves — the two wait -> arm -> issue chains overlap, and this production paces the tile.  Each is a WHOLE warp running the loop
     // converged with one elected lane issuing (see elect_one in sat_common.cuh): issued from `if (lane == 0)` code each
     // bulk copy paid register->uniform moves and an indexed walk over the launch descriptor.  Running cursors: no divisions.
     auto stream_half = [&](const bool wside) {
@@ -182,7 +174,7 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
         uint32_t par = 1u;                      // parity of empty[st] that means "free" (fresh barrier: the first pass is free)
         if (wside && L.pdl && L.w_dynamic) pdl_wait();   // the weight operand was written by the preceding kernel
         for (int it = 0; it < nkb; ++it) {
-            if (it >= S) mbar_wait(&empty[st], par);
+            if (it >= S) mbar_wait_mma(&empty[st], par);
             if (elect_one()) {
                 const uint32_t bar = bar0 + 8u * (uint32_t)st;
                 asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -206,10 +198,14 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
             }
         }
     };
-    constexpr int kXWarp = kLinThreads / 32 - 1;   // warp 9
-    if (warp == 0 && xpa) {
+    if (warp == kTmaWarp && xpa) {
         stream_half(true);
-    } else if (warp == 0) {
+    } else if (warp == kXWarp) {
+        if (xpa) {   // (this warp waited for the predecessor above)
+            if (lane == 0) tl_go(L.tl);
+            stream_half(false);
+        }
+    } else if (warp == kTmaWarp) {
         // ===================== TMA producer: one 32 KB bulk copy per stage =====================
         if (lane == 0) {
             const uint8_t* src = P.wpack + ((size_t)n_tile * P.k_blocks + kb0) * kWStageBytes;
@@ -253,10 +249,7 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
                 if (!L.pdl) for (int it = 0; it < pre; ++it) load_w(it);
                 const long long t0 = clock64();
                 while (ld_acquire_gpu(P.xbar + 1) == gen0) {
-                    if (clock64() - t0 > SAT_SPIN_LIMIT_CYCLES) {
-                        printf("sat_b200: activation pack barrier timed out (block %d)\n", (int)blockIdx.x);
-                        __trap();
-                    }
+                    if (clock64() - t0 > SAT_SPIN_LIMIT_CYCLES) __trap();   // activation pack barrier
                 }
                 fence_proxy_async_global();
                 trace_stamp(L.dbg, 3);
@@ -265,70 +258,19 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
             for (int it = (xtma || L.pdl) ? pre : 0; it < nkb; ++it) {
                 const int s = it % S;
                 const uint32_t ph = (uint32_t)(it / S) & 1u;
-                mbar_wait(&empty[s], ph ^ 1u);
+                mbar_wait_mma(&empty[s], ph ^ 1u);
                 load_w(it);
                 if (xtma) load_x(it);
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // The whole warp runs the loop (converged: all lanes wait on the stage barriers) and one elected lane issues the
-        // MMAs and the commits: their descriptors then live in uniform registers (see elect_one in sat_common.cuh).
-        {
-            const uint32_t idesc = umma_idesc_bf16(kTileN, N);
-            const uint32_t lbo = mode == 0 ? 128u : 16u;
-            const uint32_t layout = mode == 0 ? 0u : 2u;
-            const uint32_t kstep16 = (mode == 0 ? 256u : 32u) >> 4;  // descriptor address units (16 B) per UMMA K (=16 bf16)
-            const uint64_t dzero = umma_smem_desc(0u, lbo, 1024, layout);   // descriptor of byte address 0; the start address is added
-            const uint32_t stage0 = smem_u32(stage_base);
-            const uint32_t tmem_acc = __shfl_sync(0xffffffffu, tmem_d, 0);
-            int s = 0;
-            uint32_t ph = 0u;
-#pragma unroll 1
-            for (int it = 0; it < nkb; ++it) {
-                mbar_wait(&full_w[s], ph);
-                if (it == 0 && lane == 0) trace_stamp(L.dbg, 4);
-                mbar_wait(&full_x[s], ph);
-                if (it == 0 && lane == 0) trace_stamp(L.dbg, 5);
-                tc_fence_after();
-                if (elect_one()) {
-                    // (14-bit start-address field: in a cluster launch a shared-memory address carries the CTA's rank in
-                    // its high bits, which must not leak into the descriptor's other fields)
-                    const uint32_t wb = stage0 + (uint32_t)s * stage_bytes;
-                    uint64_t a_hi = dzero + (uint64_t)((wb >> 4) & 0x3FFFu);
-                    uint64_t a_lo = dzero + (uint64_t)(((wb + kWHalfBytes) >> 4) & 0x3FFFu);
-                    uint64_t b_hi = dzero + (uint64_t)(((wb + kWStageBytes) >> 4) & 0x3FFFu);
-                    uint64_t b_lo = dzero + (uint64_t)(((wb + kWStageBytes + x_half_bytes) >> 4) & 0x3FFFu);
-#pragma unroll
-                    for (int kk = 0; kk < kBK / 16; ++kk) {
-                        umma_f16(tmem_acc, a_hi, b_hi, idesc, (it | kk) != 0 ? 1u : 0u);
-                        umma_f16(tmem_acc, a_lo, b_hi, idesc, 1u);
-                        umma_f16(tmem_acc, a_hi, b_lo, idesc, 1u);
-                        a_hi += kstep16; a_lo += kstep16; b_hi += kstep16; b_lo += kstep16;
-                    }
-                    umma_commit(&empty[s]);  // frees the stage once these MMAs have read it
-                    if (it == nkb - 1) {
-                        umma_commit(tmem_full);
-                        trace_stamp(L.dbg, 6);
-                    }
-                }
-                __syncwarp();
-                if (++s == S) { s = 0; ph ^= 1u; }
-            }
-            if (L.tl) { mbar_wait(tmem_full, 0); if (lane == 0) tl_main_done(L.tl); }
-        }
-    } else {
-        // ===================== X producers (warps 2..9), then epilogue =====================
+    } else if (warp < kTmaWarp) {
+        // ===================== consumer warpgroups (warps 0..7): X producers, MMA, epilogue =====================
         // The fp32 sources of X are L2 resident; their latency is hidden by keeping the loads of the
         // NEXT chunk in flight while the current one is converted and stored.
-        const int pt = threadIdx.x - 64;  // 0..255
+        const int pt = threadIdx.x;  // 0..255
         if (pt == 0) trace_stamp(L.dbg, 1);
-        if (xpa && warp == kXWarp) {      // (this warp waited for the predecessor above, like every epilogue warp)
-            if (lane == 0) tl_go(L.tl);
-            stream_half(false);
-        }
         if (xpre) {
-            // ---- cooperative pre-pass: this problem's CTAs convert X (fp32 -> bf16 hi/lo UMMA tiles) ONCE
+            // ---- cooperative pre-pass: this problem's CTAs convert X (fp32 -> bf16 hi/lo MMA operand tiles) ONCE
             // into global scratch; consecutive threads take consecutive 8-element groups of a row (coalesced).
             const int kgroups = P.k_blocks * 8;
             const int utot = P.n_row_tiles * N * kgroups;
@@ -340,7 +282,7 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
                 uint4 hi, lo;
                 split_bf16x8(a, c, hi, lo);
                 uint8_t* dst = P.xpack + ((size_t)rt2 * P.k_blocks + (kgk >> 3)) * x_stage_bytes +
-                               umma_tile_off(mode, r, kgk & 7);
+                               mma_tile_off(mode, r, kgk & 7);
                 *reinterpret_cast<uint4*>(dst) = hi;
                 *reinterpret_cast<uint4*>(dst + x_half_bytes) = lo;
             }
@@ -372,37 +314,9 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
                 }
             }
         };
-        XChunk cur, nxt;
-        if (total > 0) load_chunk(0, cur);
-        for (int g = 0; g < total; ++g) {
-            const int it = g / JC, jc = g - it * JC;
-            const int s = it % S;
-            if (g + 1 < total) load_chunk(g + 1, nxt);
-            if (jc == 0) mbar_wait(&empty[s], ((uint32_t)(it / S) & 1u) ^ 1u);
-            uint8_t* xh = stage_base + (size_t)s * stage_bytes + kWStageBytes;
-            uint8_t* xl = xh + x_half_bytes;
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int u = pt + kLinProducers * (jc * 2 + e);
-                if (u < units) {
-                    const int kg = u / N, r = u - kg * N;
-                    uint4 hi, lo;
-                    split_bf16x8(cur.a[e], cur.c[e], hi, lo);
-                    const uint32_t off = umma_tile_off(mode, r, kg);
-                    *reinterpret_cast<uint4*>(xh + off) = hi;
-                    *reinterpret_cast<uint4*>(xl + off) = lo;
-                }
-            }
-            if (jc == JC - 1) {
-                fence_proxy_async_smem();
-                mbar_arrive(&full_x[s]);
-            }
-            cur = nxt;
-        }
-
         // ---- epilogue.  Code that runs once per launch is fetched cold (the instruction caches do not survive
         // the other kernels of a step), and a cold straight-line epilogue costs several microseconds on the
-        // critical path.  In the TMA-fed modes these warps are idle while the main loop streams, so they first
+        // critical path.  In the TMA-fed modes these warps would wait for the first stages anyway, so they first
         // run the epilogue once "dry" (same instructions, loads from harmless addresses, no stores, no
         // synchronisation with other CTAs) purely to pull its code into the instruction caches.
         // (the bias does not depend on the accumulator: fetch it while the main loop runs)
@@ -425,9 +339,9 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
         // the row loop is skipped when the arg-max is all that is wanted from this layer
         const bool row_loop = epi == kEpiLstm || out != nullptr || out_pa != nullptr;
         unsigned long long* const am_key = do_am ? P.am_key + (size_t)(rt * P.n_tiles + n_tile) * N : nullptr;
-        // arg-max layers fold the bias into the tile as it leaves TMEM (this thread's TMEM lane = one output): the
-        // arg-max scan then reads finished values; the row loop must not add it again
-        const float bias_fold = (do_am && P.bias) ? P.bias[n_tile * kTileN + (warp & 3) * 32 + lane] : 0.f;
+        // arg-max layers fold the bias into the tile as it leaves the accumulator: the arg-max scan then reads
+        // finished values; the row loop must not add it again
+        const float* const bias_fold = (do_am && P.bias) ? P.bias + n_tile * kTileN : nullptr;
         // LSTM: c_prev of the (at most two) rows this thread finishes, fetched while the main loop runs
         float cpre[2] = {0.f, 0.f};
         if (epi == kEpiLstm && unit < Hh) {
@@ -444,24 +358,70 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
         for (int pass = (xtma && L.warm_epilogue && (!row_loop || hi - lo <= 8 * kLinProducers)) ? 0 : 1; pass < 2; ++pass) {
             const bool dry = pass == 0;
             if (!dry) {
-                // ---- part 1: accumulator tile TMEM -> shared memory (two warps per TMEM lane quadrant).
-                // tile_s[col][n] (fp32, n fastest) lives in the idle pipeline stages: every TMA write has landed
-                // and every MMA has read its operands once tmem_full fires.
-                const int q = warp & 3;               // TMEM lane quadrant this warp may access
-                const int half = (warp - 2) >> 2;     // 0 or 1
-                const int nl = q * 32 + lane;         // output feature within the tile (TMEM lane)
-                mbar_wait(tmem_full, 0);
-                tc_fence_after();
-                if (pt == 0) trace_stamp(L.dbg, 7);
-                const uint32_t taddr = tmem_d + ((uint32_t)(q * 32) << 16);
+                // ---- main loop: per K block, both warpgroups issue their 64 x N x 64 share of the three products
+                AccTile<NT> acc;
+                const uint32_t stage0 = smem_u32(stage_base);
+                if (xtma) {
+                    int s = 0;
+                    uint32_t ph = 0u;
 #pragma unroll 1
-                for (int c0 = half * 16; c0 < N; c0 += 32) {
-                    float v[16];
-                    tmem_ld16(taddr + (uint32_t)c0, v);
+                    for (int it = 0; it < nkb; ++it) {
+                        mbar_wait_mma(&full_w[s], ph);
+                        if (it == 0 && pt == 0) trace_stamp(L.dbg, 4);
+                        mbar_wait_mma(&full_x[s], ph);
+                        if (it == 0 && pt == 0) trace_stamp(L.dbg, 5);
+                        mma_kblock(acc, stage0 + (uint32_t)s * stage_bytes, x_half_bytes, mode, it == 0);
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&empty[s]);   // frees the stage: this warp's MMAs have read it
+                        if (++s == S) { s = 0; ph ^= 1u; }
+                    }
+                } else {
+                    // X converted by these warps, one K block at a time: its stage is free (this thread's MMAs on
+                    // it completed S blocks ago; with one stage, the barrier below waits for the other warpgroup)
+                    XChunk cur, nxt;
+                    load_chunk(0, cur);
+#pragma unroll 1
+                    for (int g = 0; g < total; ++g) {
+                        const int it = g / JC, jc = g - it * JC;
+                        const int s = it % S;
+                        if (g + 1 < total) load_chunk(g + 1, nxt);
+                        if (jc == 0 && S == 1 && it > 0) named_bar_sync(1, kLinProducers);
+                        uint8_t* xh = stage_base + (size_t)s * stage_bytes + kWStageBytes;
+                        uint8_t* xl = xh + x_half_bytes;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) tile_s[(c0 + j) * kTileN + nl] = v[j] + bias_fold;
+                        for (int e = 0; e < 2; ++e) {
+                            const int uu = pt + kLinProducers * (jc * 2 + e);
+                            if (uu < units) {
+                                const int kg = uu / N, r = uu - kg * N;
+                                uint4 xhi, xlo;
+                                split_bf16x8(cur.a[e], cur.c[e], xhi, xlo);
+                                const uint32_t off = mma_tile_off(mode, r, kg);
+                                *reinterpret_cast<uint4*>(xh + off) = xhi;
+                                *reinterpret_cast<uint4*>(xl + off) = xlo;
+                            }
+                        }
+                        if (jc == JC - 1) {
+                            fence_proxy_async_smem();                 // X stores -> visible to the wgmma reads
+                            named_bar_sync(1, kLinProducers);         // every consumer warp has stored its part
+                            mbar_wait_mma(&full_w[s], (uint32_t)(it / S) & 1u);
+                            if (it == 0 && pt == 0) trace_stamp(L.dbg, 4);
+                            mma_kblock(acc, stage0 + (uint32_t)s * stage_bytes, x_half_bytes, mode, it == 0);
+                            __syncwarp();
+                            if (lane == 0) mbar_arrive(&empty[s]);
+                        }
+                        cur = nxt;
+                    }
                 }
-                tc_fence_before();
+                if (pt == 0) trace_stamp(L.dbg, 6);
+                if (L.tl && pt == 0) tl_main_done(L.tl);
+                // ---- part 1: accumulator tile -> shared memory.  tile_s[col][n] (fp32, n fastest) lives in the idle
+                // pipeline stages: every TMA write has landed, and every MMA has read its operands once both
+                // warpgroups are past this barrier.
+                named_bar_sync(1, kLinProducers);
+                if (pt == 0) trace_stamp(L.dbg, 7);
+                acc_for_each(acc, N, [&](int m, int n, float v) {
+                    tile_s[n * kTileN + m] = bias_fold ? v + bias_fold[m] : v;
+                });
                 // ---- split-K partials meet through distributed shared memory.  The `splits` CTAs of a tile form
                 // one thread-block cluster; after the cluster barrier CTA `split` sums rows [lo, hi) of all
                 // partial tiles in fixed rank order (bit-reproducible), applies the fused epilogue and writes
@@ -642,10 +602,7 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
                         } else if (local < P.rows) {             // (CTAs with no row to finish leave at once)
                             const long long t0 = clock64();
                             while (ld_acquire_gpu(P.am_ctr + 1) == am_gen0) {
-                                if (clock64() - t0 > SAT_SPIN_LIMIT_CYCLES) {
-                                    printf("sat_b200: arg-max rendezvous timed out (block %d)\n", (int)blockIdx.x);
-                                    __trap();
-                                }
+                                if (clock64() - t0 > SAT_SPIN_LIMIT_CYCLES) __trap();   // arg-max rendezvous
                             }
                         }
                         trace_stamp(L.dbg, 12);
@@ -687,7 +644,7 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
                             uint4 hi4, lo4;
                             split_bf16x8(a4, c4, hi4, lo4);
                             uint8_t* dst = P.am_emb_pa + ((size_t)rt2 * (E >> 6) + (gi >> 3)) * 2 * halfb +
-                                           umma_tile_off(mode, rr, gi & 7);
+                                           mma_tile_off(mode, rr, gi & 7);
                             if (!dry) {
                                 *reinterpret_cast<uint4*>(dst) = hi4;
                                 *reinterpret_cast<uint4*>(dst + halfb) = lo4;
@@ -699,26 +656,21 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_umma_kernel(const __grid_c
             }
         }
     }
-    if (warp < 2 && P.splits > 1) {   // the TMA / MMA warps join the cluster rendezvous of the epilogue
+    if (warp >= kTmaWarp && P.splits > 1) {   // the TMA warps join the cluster rendezvous of the epilogue
         __syncwarp();
         cluster_sync_all();
         cluster_arrive_relaxed();
     }
-    if (threadIdx.x == 64) trace_stamp(L.dbg, 9);
+    if (threadIdx.x == 0) trace_stamp(L.dbg, 9);
     if (P.splits > 1) cluster_wait();   // peers may still be reading this CTA's tile
 
     __syncthreads();
     if (threadIdx.x == 0) { trace_stamp(L.dbg, 10); tl_end(L.tl); }
-    if (warp == 1) {
-        __syncwarp();
-        tc_fence_after();
-        tmem_dealloc(tmem_d, tmem_cols);
-    }
 }
 
 // -------------------------------------------------- SIMT bring-up kernel
 // Same math on CUDA cores from the same packed weights (w = hi + lo).  Used by
-// the tests to cross-check the tcgen05 path and its packing; selected with
+// the tests to cross-check the wgmma path and its packing; selected with
 // sat_set_option("gemm", 0).  Grid: one CTA per (n_tile, 16-row group).
 __global__ void __launch_bounds__(128) lin_simt_kernel(const __grid_constant__ LinLaunch L) {
     __shared__ float xs[16][kBK + 1];
@@ -748,7 +700,7 @@ __global__ void __launch_bounds__(128) lin_simt_kernel(const __grid_constant__ L
         __syncthreads();
         const uint8_t* tile = P.wpack + ((size_t)n_tile * P.k_blocks + kb) * kWStageBytes;
         for (int kg = 0; kg < 8; ++kg) {
-            const uint32_t off = umma_tile_off(mode, r, kg);
+            const uint32_t off = mma_tile_off(mode, r, kg);
             const uint4 hi = *reinterpret_cast<const uint4*>(tile + off);
             const uint4 lo = *reinterpret_cast<const uint4*>(tile + kWHalfBytes + off);
             const uint32_t hh[4] = {hi.x, hi.y, hi.z, hi.w}, ll[4] = {lo.x, lo.y, lo.z, lo.w};
@@ -788,7 +740,7 @@ __global__ void __launch_bounds__(128) lin_simt_kernel(const __grid_constant__ L
 
 // ---------------------------------------------------- one-time weight repack
 // TF kernel [K, n_out] fp32 row-major (tf.layers.dense, utils/nn.py:96-105) ->
-// packed bf16 hi/lo UMMA tiles.  perm_H > 0 selects the LSTM gate interleave:
+// packed bf16 hi/lo MMA operand tiles.  perm_H > 0 selects the LSTM gate interleave:
 // packed output p = unit*4 + gate  <->  TF column gate*H + unit (split order i,j,f,o).
 __global__ void repack_weight_kernel(const float* __restrict__ w, int K, int n_out, int perm_H, uint8_t* wpack,
                                      int k_blocks, int n_tiles, int mode, DropSpec drop, int pdl) {
@@ -816,7 +768,7 @@ __global__ void repack_weight_kernel(const float* __restrict__ w, int K, int n_o
         uint4 hi, lo;
         split_bf16x8(make_float4(x[0], x[1], x[2], x[3]), make_float4(x[4], x[5], x[6], x[7]), hi, lo);
         uint8_t* tile = wpack + ((size_t)nt * k_blocks + kb) * kWStageBytes;
-        const uint32_t off = umma_tile_off(mode, r, kg);
+        const uint32_t off = mma_tile_off(mode, r, kg);
         *reinterpret_cast<uint4*>(tile + off) = hi;
         *reinterpret_cast<uint4*>(tile + kWHalfBytes + off) = lo;
     }
@@ -871,7 +823,7 @@ __global__ void pack_rows_kernel(const PackJobs J) {
             split_bf16x8(a, c, hi, lo);
             const int rt = b / jb.row_tile, r = b - rt * jb.row_tile;
             const int kbs = jb.k_blocks > 0 ? jb.k_blocks : (jb.width >> 6);
-            uint8_t* dst = jb.pa + ((size_t)rt * kbs + (g >> 3)) * 2 * half + umma_tile_off(J.mode, r, g & 7);
+            uint8_t* dst = jb.pa + ((size_t)rt * kbs + (g >> 3)) * 2 * half + mma_tile_off(J.mode, r, g & 7);
             *reinterpret_cast<uint4*>(dst) = hi;
             *reinterpret_cast<uint4*>(dst + half) = lo;
         }
@@ -906,7 +858,7 @@ cudaError_t pack_rows_launch(const PackJob* jobs, int njobs, int layout_mode, cu
         total = max(total, nrt * jobs[i].row_tile * (jobs[i].width >> 3));
     }
     int grid = (total + 255) / 256;
-    if (grid > 148 * 8) grid = 148 * 8;   // every thread converts a few 32-byte groups: short dependent chains
+    if (grid > device_sm_count() * 8) grid = device_sm_count() * 8;   // every thread converts a few 32-byte groups: short dependent chains
     if (grid < 1) grid = 1;
     if (pdl) return launch_serialized(pack_rows_kernel, grid, 256, st, J);
     pack_rows_kernel<<<grid, 256, 0, st>>>(J);
@@ -914,7 +866,22 @@ cudaError_t pack_rows_launch(const PackJob* jobs, int njobs, int layout_mode, cu
 }
 
 // ------------------------------------------------------------ host side
+int device_sm_count() {
+    static int cached[64] = {0};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+    if (cached[dev] == 0 && cudaDeviceGetAttribute(&cached[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+        cudaGetLastError();
+        return 132;
+    }
+    return cached[dev];
+}
+
 static int g_smem_optin = 0;
+
+static void (*const g_lin_kernels[kMaxRowTile / 16])(LinLaunch) = {
+    lin_mma_kernel<1>, lin_mma_kernel<2>, lin_mma_kernel<3>, lin_mma_kernel<4>,
+    lin_mma_kernel<5>, lin_mma_kernel<6>, lin_mma_kernel<7>, lin_mma_kernel<8>};
 
 cudaError_t lin_init_attrs() {
     int dev = 0;
@@ -922,7 +889,11 @@ cudaError_t lin_init_attrs() {
     if (e != cudaSuccess) return e;
     e = cudaDeviceGetAttribute(&g_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(lin_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin);
+    for (auto k : g_lin_kernels) {
+        e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 size_t lin_smem_bytes(int row_tile, int stages) {
@@ -953,6 +924,9 @@ cudaError_t lin_launch(const LinLaunch& L, cudaStream_t st, bool use_simt) {
     for (int i = 0; i < L.nprob; ++i) {
         total += L.p[i].cta_count;
         if (L.p[i].row_tile > max_rt) max_rt = L.p[i].row_tile;
+        // (one MMA width per launch: grouped problems share the row tile, so no MMA reads past its operand)
+        if (L.p[i].row_tile % 16 || L.p[i].row_tile > kMaxRowTile || L.p[i].row_tile != L.p[0].row_tile)
+            return cudaErrorInvalidValue;
     }
     const size_t smem = lin_smem_bytes(max_rt, L.stages);
     // every problem of a launch uses the same split factor: the `splits` CTAs of a tile are one cluster
@@ -985,7 +959,7 @@ cudaError_t lin_launch(const LinLaunch& L, cudaStream_t st, bool use_simt) {
     }
     cfg.attrs = at;
     cfg.numAttrs = na;
-    return cudaLaunchKernelEx(&cfg, lin_umma_kernel, L);
+    return cudaLaunchKernelEx(&cfg, g_lin_kernels[max_rt / 16 - 1], L);
 }
 
 cudaError_t lin_repack_weight(const float* w_tf, int K, int n_out, int perm_H, uint8_t* wpack, int layout_mode,

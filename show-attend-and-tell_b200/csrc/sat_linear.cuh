@@ -1,6 +1,6 @@
 // sat_linear.cuh — descriptors of the small-batch dense layer kernels
 // (tf.layers.dense / LSTMCell matmul of the reference: utils/nn.py:85-105,
-// model.py:276-279, 438-459) as executed on sm_100a.
+// model.py:276-279, 438-459) as executed on sm_90a.
 #pragma once
 #include <stdint.h>
 #include <cuda_runtime.h>
@@ -9,11 +9,13 @@
 namespace sat {
 
 constexpr int kBK = 64;                                  // K elements per pipeline stage
-constexpr int kTileN = 128;                              // outputs per CTA tile (UMMA M)
+constexpr int kTileN = 128;                              // outputs per CTA tile (wgmma M of two warpgroups)
 constexpr int kWHalfBytes = kTileN * kBK * 2;            // one bf16 half (hi or lo) of a W tile
 constexpr int kWStageBytes = 2 * kWHalfBytes;            // hi + lo, contiguous in the packed image
-constexpr int kLinThreads = 320;                         // warp0 TMA, warp1 MMA, warps2-9 X-producer/epilogue
-constexpr int kLinProducers = 256;
+constexpr int kLinThreads = 320;                         // warps 0-7 MMA / X-producer / epilogue, warp 8 TMA, warp 9 X TMA
+constexpr int kLinProducers = 256;                       // the consumer warps 0-7 (two warpgroups)
+constexpr int kMaxRowTile = 128;                         // batch rows per CTA tile (wgmma N), multiple of 16: the
+                                                         // accumulator (N / 2 registers per consumer thread) fits
 constexpr int kMaxSeg = 3;
 constexpr int kMaxProb = 4;
 
@@ -36,7 +38,7 @@ struct LinSeg {
 };
 
 // A "packed activation": an fp32 [rows, width] tensor (width % 64 == 0) kept by its PRODUCER kernel in
-// the bf16 hi/lo UMMA operand image  [n_row_tiles][width/64][hi|lo][row_tile x 64 bf16]  so that the
+// the bf16 hi/lo MMA operand image  [n_row_tiles][width/64][hi|lo][row_tile x 64 bf16]  so that the
 // consuming dense layer fetches its X stages by TMA with no conversion pass.
 __host__ __device__ __forceinline__ size_t pa_stage_bytes(int row_tile) { return (size_t)row_tile * kBK * 2 * 2; }
 
@@ -46,12 +48,12 @@ struct LinProblem {
     int K;          // sum of widths
     int k_blocks;   // ceil(K / kBK)
     int rows;       // valid activation rows (batch)
-    int row_tile;   // activation rows per CTA = UMMA N, multiple of 16, <= 256
+    int row_tile;   // activation rows per CTA = wgmma N, multiple of 16, <= kMaxRowTile
     int n_row_tiles;
     int n_out;      // valid outputs
     int n_tiles;    // ceil(n_out / 128)
     int splits;     // split-K factor = thread-block cluster size (1, 2, 4 or 8)
-    const uint8_t* wpack;  // [n_tiles][k_blocks][hi|lo][128 x 64 bf16, canonical UMMA K-major layout]
+    const uint8_t* wpack;  // [n_tiles][k_blocks][hi|lo][128 x 64 bf16, canonical K-major MMA operand layout]
     const float* bias;     // packed output order, n_tiles*128 entries (zero padded); may be null for kEpiNone
     uint8_t* xpack;        // x_mode 1: packed activations [n_row_tiles][k_blocks][hi|lo][row_tile x 64 bf16]
     unsigned* xbar;        // x_mode 1: grid barrier {count, generation}
@@ -100,7 +102,7 @@ struct LinLaunch {
 
 // byte offset of the 16-byte group (row r, k-group kg in [0,8)) inside a [rows x 64] bf16
 // K-major operand tile.  Both modes place 8-row groups 1024 B apart.
-__host__ __device__ __forceinline__ uint32_t umma_tile_off(int mode, int r, int kg) {
+__host__ __device__ __forceinline__ uint32_t mma_tile_off(int mode, int r, int kg) {
     return mode == 0 ? (uint32_t)((r >> 3) * 1024 + kg * 128 + (r & 7) * 16)
                      : (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((kg ^ (r & 7)) * 16));
 }
@@ -111,7 +113,7 @@ __device__ __forceinline__ void pa_store(uint8_t* pa, int mode, int row_tile, in
     const int rt = b / row_tile, r = b - rt * row_tile;
     const int kb = col >> 6, kg = (col & 63) >> 3, e = col & 7;
     const size_t half = (size_t)row_tile * kBK * 2;
-    uint8_t* dst = pa + ((size_t)rt * kblocks + kb) * 2 * half + umma_tile_off(mode, r, kg) + e * 2;
+    uint8_t* dst = pa + ((size_t)rt * kblocks + kb) * 2 * half + mma_tile_off(mode, r, kg) + e * 2;
     const __nv_bfloat16 h = __float2bfloat16_rn(v);
     const __nv_bfloat16 l = __float2bfloat16_rn(v - __bfloat162float(h));
     *reinterpret_cast<__nv_bfloat16*>(dst) = h;
@@ -122,7 +124,7 @@ __device__ __forceinline__ void pa_store4(uint8_t* pa, int mode, int row_tile, i
     const int rt = b / row_tile, r = b - rt * row_tile;
     const int kb = col >> 6, kg = (col & 63) >> 3, e = col & 7;
     const size_t half = (size_t)row_tile * kBK * 2;
-    uint8_t* dst = pa + ((size_t)rt * kblocks + kb) * 2 * half + umma_tile_off(mode, r, kg) + e * 2;
+    uint8_t* dst = pa + ((size_t)rt * kblocks + kb) * 2 * half + mma_tile_off(mode, r, kg) + e * 2;
     uint32_t h[2], l[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -225,9 +227,9 @@ cudaError_t pack_rows_launch(const PackJob* jobs, int njobs, int layout_mode, cu
 // grid-wide arrival counters in global memory; what a separate launch per layer cannot do and this does: every CTA is
 // resident from the start, and its TMA lane streams the (immutable) weights of its next tile into the pipeline
 // stages as they free up, i.e. under the epilogue and the rendezvous of the current phase.
-//   * all operands arrive packed (x_mode 2 of lin_umma_kernel), one row tile (rows <= row_tile <= 64);
+//   * all operands arrive packed (x_mode 2 of lin_mma_kernel), one row tile (rows <= row_tile <= 64);
 //   * split-K partial tiles meet in a global (L2 resident) scratch buffer behind a per-tile arrival counter, summed in
-//     fixed split order (bit-identical to the cluster / DSMEM reduction of lin_umma_kernel);
+//     fixed split order (bit-identical to the cluster / DSMEM reduction of lin_mma_kernel);
 //   * arg-max of the vocabulary phase: one atomicMax per (row, tile) on the ordered 64-bit key; every CTA but the
 //     last to arrive exits at once (its SM is free for the next launch); the last arriver records the words and packs
 //     their embedding rows for the next step.
@@ -253,7 +255,7 @@ struct LinChain {
                            // one cluster) exchange their partial tiles through distributed shared memory behind a pair
                            // of mbarriers per phase; 1: through `scratch` in L2 behind the tile counters
     unsigned long long* tl;   // optional timeline cells (see tl_begin)
-    unsigned long long* dbg;  // optional [grid][16] per-CTA stamps (tools/trace_chain.py)
+    unsigned long long* dbg;  // optional [grid][16] per-CTA stamps
     int dbg_mode;             // 0: phase milestones; 1: phase 0 per K block (slots 0-7 operands landed, 8-15 weight copy issued)
 };
 size_t lin_chain_smem_bytes(int row_tile, int stages);
@@ -269,5 +271,6 @@ cudaError_t lin_repack_weight(const float* w_tf, int K, int n_out, int perm_H, u
                               cudaStream_t st, const DropSpec* drop = nullptr, int pdl = 0);
 cudaError_t lin_repack_bias(const float* b_tf, int n_out, int perm_H, float* bias_packed, cudaStream_t st);
 cudaError_t lin_init_attrs();
+int device_sm_count();   // SMs of the current device (sizes grids and split factors)
 
 }  // namespace sat

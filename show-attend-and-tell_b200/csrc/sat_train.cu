@@ -203,10 +203,10 @@ cudaError_t sgemm(cudaStream_t st, bool ta, bool tb, int M, int N, int K, const 
     dim3 grid((N + GN - 1) / GN, (M + GM - 1) / GM, 1);
     int kchunk = K;
     const int tiles = grid.x * grid.y;
-    if (tiles < 148 && K >= 512) {
+    if (tiles < sat::device_sm_count() && K >= 512) {
         // few output tiles (batch-sized M, or weight gradients with a huge K): split K over the SMs and sum
         // with atomics.  A non-accumulating product starts from a zeroed C (ldc == N: contiguous).
-        int z = (296 + tiles - 1) / tiles;
+        int z = (2 * sat::device_sm_count() + tiles - 1) / tiles;
         if (z > K / 128) z = K / 128;
         if (z < 1) z = 1;
         kchunk = ((K + z - 1) / z + GK - 1) / GK * GK;
@@ -330,7 +330,7 @@ __global__ void colsum_kernel(float* db, const float* dx, int rows, int cols, co
 __global__ void concat3_drop_kernel(float* out, int ldo, const float* a, int na, const float* b, int nb, const float* c, int nc,
                                     int ndrop, int rows, const unsigned long long* seedp, unsigned long long stream, float keep,
                                     int rows_per_step, uint8_t* pa, int pa_mode, int pa_row_tile) {
-    // pa (optional): the row also goes out as a packed operand of the tcgen05 dense kernel (row tile pa_row_tile, width
+    // pa (optional): the row also goes out as a packed operand of the wgmma dense kernel (row tile pa_row_tile, width
     // = cols, a multiple of 64): the product that consumes it needs no packing launch of its own
     pdl_enter();
     const unsigned long long seed = *seedp;
@@ -1066,7 +1066,7 @@ struct TrainState {
           *dlin = nullptr, *dz = nullptr, *demb = nullptr, *dalpha = nullptr, *dtemp = nullptr, *dq = nullptr, *dhd = nullptr,
           *dbuf = nullptr;
     // tensor-core path of attend/fc_1a (forward + weight gradient: ~25 % of the step's time on CUDA cores): the
-    // operands in the packed layouts of the tcgen05 dense kernel
+    // operands in the packed layouts of the wgmma dense kernel
     uint8_t *tc_xpa = nullptr, *tc_wbig = nullptr, *tc_w1a = nullptr;   // packed rows / packed [BL x A] "weight" / packed W1a
     float* tc_b1a = nullptr;
     bool tc_ok = false;
@@ -1254,7 +1254,7 @@ extern "C" int sat_train_init(sat_handle* h, int32_t B, int32_t T, float fc_drop
             l.var_w = vw[i]; l.var_b = vb[i]; l.K = (int)Ks[i]; l.N = (int)Ns[i];
             // (the 1-layer variants of attend / decode stay on the CUDA-core products: they are not the shipped graph)
             const bool used = i == 1 || (i == 0 ? att2 : dec2);
-            l.fwd = used && (Ks[i] % 64 == 0) && s->tc_rt <= 256;
+            l.fwd = used && (Ks[i] % 64 == 0) && s->tc_rt <= sat::kMaxRowTile;
             l.dx = l.fwd && (Ns[i] % 64 == 0);
             float* f = nullptr;
             const size_t npad = (Ns[i] + 127) / 128 * 128, kpad = (Ks[i] + 127) / 128 * 128;
@@ -1429,10 +1429,10 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
     auto tc_splits = [&](int n_out, int K) {
         const int tiles = (n_out + 127) / 128;
         int sp = 1;
-        while (sp * 2 <= 8 && tiles * sp * 2 <= 148 && sp * 2 <= K / 64) sp *= 2;
+        while (sp * 2 <= 8 && tiles * sp * 2 <= sat::device_sm_count() && sp * 2 <= K / 64) sp *= 2;
         return sp;
     };
-    // y[B, N] = epi(x[B, K] W + b) on the tcgen05 kernel; false if this layer / shape stays on the CUDA-core path
+    // y[B, N] = epi(x[B, K] W + b) on the wgmma kernel; false if this layer / shape stays on the CUDA-core path
     auto tc_fwd = [&](int li, const float* x, int epi, float* y, int* rc) -> bool {
         TrainState::TcLayer& l = s->tcl[li];
         if (!tcb || !l.fwd) return false;
@@ -1485,7 +1485,7 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
     auto all_splits = [&](int n_out, int K) {
         const int tiles = ((n_out + 127) / 128) * (s->all_rows / (s->all_rt > 0 ? s->all_rt : 1));
         int sp = 1;
-        while (sp * 2 <= 8 && tiles * sp * 2 <= 148 && sp * 2 <= K / 64) sp *= 2;
+        while (sp * 2 <= 8 && tiles * sp * 2 <= sat::device_sm_count() && sp * 2 <= K / 64) sp *= 2;
         return sp;
     };
     // scorer: fused one-pass kernels when the rows are float4-addressable (every buffer involved is a cudaMalloc'd
@@ -1497,15 +1497,15 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
     int ab_chunks = 1, ab_rows = L, ab_wave = 0;
     {
         const int gx = (A / 4 + kAbCT - 1) / kAbCT;
-        ab_chunks = (148 * 4 + B * gx - 1) / (B * gx > 0 ? B * gx : 1);   // about four CTAs per SM
+        ab_chunks = (sat::device_sm_count() * 4 + B * gx - 1) / (B * gx > 0 ? B * gx : 1);   // about four CTAs per SM
         if (ab_chunks > (L + 15) / 16) ab_chunks = (L + 15) / 16;
         if (ab_chunks < 1) ab_chunks = 1;
-        // SAT_TRAIN_ATTBWD_WAVE=1 (experiment, see DESIGN.md section 7): the 64-register build of the kernel and as many row
-        // chunks as fit ONE resident wave (the default shape is 1.44 waves of 3 CTAs per SM at config 4)
+        // SAT_TRAIN_ATTBWD_WAVE=1 (experiment, off by default): the 64-register build of the kernel and as many row
+        // chunks as fit ONE resident wave, which trades registers per thread for the absence of a partly filled tail wave
         static const int one_wave = []() { const char* e = getenv("SAT_TRAIN_ATTBWD_WAVE"); return (e && e[0] == '1') ? 1 : 0; }();
         ab_wave = one_wave;
         if (one_wave) {
-            int occ = 0, sms = 148, dev = 0;
+            int occ = 0, sms = sat::device_sm_count(), dev = 0;
             cudaGetDevice(&dev);
             cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
             if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, att_bwd_fused_wave_kernel, kAbRG * kAbCT, 0) != cudaSuccess || occ < 1) occ = 1;
@@ -1536,7 +1536,7 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
             launch_k(dropout2d_kernel, GRID1D((size_t)BL * D), 256, st, s->ctxd, D, contexts, D, BL, D, seed, ST(t, 0), kf, 0);
             launch_k(rowdot_kernel, (BL * 32 + 255) / 256, 256, st, s->e, s->ctxd, P(vA1aW), BL, D);
         } else if (side_f) {
-        } else if (tc) {   // T1 = tanh(drop(ctx) W1a + b1a) on the tcgen05 dense kernel: the context dropout is applied while the
+        } else if (tc) {   // T1 = tanh(drop(ctx) W1a + b1a) on the wgmma dense kernel: the context dropout is applied while the
                     // rows are packed (no fp32 dropped copy), bias + tanh fused in the epilogue
             sat::PackJob job{contexts, nullptr, D, D, BL, 128, s->tc_xpa};
             const sat::DropSpec drop{seed, ST(t, 0), kf};
@@ -1628,7 +1628,7 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
         if (s->regularised[v]) {
             const size_t n = (size_t)s->rows[v] * s->cols[v];
             const int g = (int)((n / 4 + 1023) / 1024);   // about four float4 per thread
-            launch_k(sumsq_kernel, g < 1 ? 1 : (g > 148 * 8 ? 148 * 8 : g), 256, st, P(v), n, 0.5f * s->reg_scale, s->loss_acc + 3);
+            launch_k(sumsq_kernel, g < 1 ? 1 : (g > sat::device_sm_count() * 8 ? sat::device_sm_count() * 8 : g), 256, st, P(v), n, 0.5f * s->reg_scale, s->loss_acc + 3);
         }
 
     // ------------------------------------------------------------ backward through time
@@ -1759,7 +1759,7 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
             TCK(sat::lin_repack_weight(dy[i], TB, l.N, 0, s->tc_sw, lmode, st, nullptr, PDLK));
             int sp = 1;
             const int tiles = ((l.N + 127) / 128) * ((l.K + 127) / 128);
-            while (sp * 2 <= 8 && tiles * sp * 2 <= 148) sp *= 2;
+            while (sp * 2 <= 8 && tiles * sp * 2 <= sat::device_sm_count()) sp *= 2;
             TRET(sat_dense_packed(s->handle, s->tc_sx, l.K, 128, TB, s->tc_sw, nullptr, l.N, sat::kEpiNone, Gd(l.var_w), l.N, 1, sp, st, 1));
             launch_k(colsum_kernel, dim3((l.N + 127) / 128, (TB + 255) / 256), 128, st, Gd(l.var_b), dy[i], TB, l.N, nullptr);
         }
@@ -1878,7 +1878,7 @@ extern "C" int sat_train_apply_opt(sat_handle* h, float* params, float* grads, f
             launch_k(axpy_kernel, GRID1D(nv), 256, st, grads + s->off[v], params + s->off[v], s->reg_scale, nv);
         }
     TCK(cudaMemsetAsync(s->loss_acc + 4, 0, sizeof(float), st));
-    launch_k(sumsq_kernel, 148 * 8, 256, st, grads, n, 1.0f, s->loss_acc + 4);   // padding entries are zero
+    launch_k(sumsq_kernel, sat::device_sm_count() * 8, 256, st, grads, n, 1.0f, s->loss_acc + 4);   // padding entries are zero
     const float clip = opt->clip_gradients, lr = opt->learning_rate;
     if (kind == SAT_OPT_ADAM) {
         const double lr_t = (double)lr * sqrt(1.0 - pow((double)opt->beta2, (double)step)) / (1.0 - pow((double)opt->beta1, (double)step));
@@ -1900,7 +1900,7 @@ extern "C" int sat_train_apply_opt(sat_handle* h, float* params, float* grads, f
 extern "C" int sat_train_fill(sat_handle* h, float* buf, float value, int64_t n, void* stream) {
     if (!h || !buf || n < 0) return sat_fail(SAT_ERR_INVALID, "sat_train_fill: bad argument");
     TCK(cudaSetDevice(sat_handle_device(h)));
-    fill_kernel<<<148 * 4, 256, 0, (cudaStream_t)stream>>>(buf, value, (size_t)n);
+    fill_kernel<<<sat::device_sm_count() * 4, 256, 0, (cudaStream_t)stream>>>(buf, value, (size_t)n);
     TCK(cudaGetLastError());
     return SAT_OK;
 }

@@ -79,7 +79,7 @@ class CaptionGenerator(object):
     def __init__(self, config, max_batch=None, device=None):
         import torch
         if not torch.cuda.is_available():
-            raise RuntimeError("sat_b200 needs an NVIDIA B200 (sm_100a): no CUDA device visible, no CPU path")
+            raise RuntimeError("sat_b200 needs an NVIDIA H100 (sm_90a): no CUDA device visible, no CPU path")
         self.torch = torch
         self.config = config
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)

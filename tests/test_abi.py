@@ -54,14 +54,14 @@ def test_create_fails_loudly_without_a_gpu(built_lib):
         assert "no CPU path" in str(e) or "CUDA" in str(e)
 
 
-def test_sass_contains_tcgen05_and_tma(built_lib):
+def test_sass_contains_wgmma_and_tma(built_lib):
     import shutil
     import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         return
     sass = subprocess.run([cuobjdump, "-sass", built_lib], stdout=subprocess.PIPE, text=True).stdout
-    assert "UTCHMMA" in sass      # tcgen05.mma
-    assert "LDTM" in sass         # tcgen05.ld
+    assert "arch = sm_90a" in sass
+    assert "HGMMA" in sass        # wgmma.mma_async
     assert "UBLKCP" in sass       # cp.async.bulk (TMA) feeds both the dense and the attention kernels
-    assert "HMMA." not in sass.replace("UTCHMMA", "")   # no legacy mma.sync path
+    assert "HMMA." not in sass    # no legacy mma.sync path

@@ -1,4 +1,4 @@
-"""tcgen05 dense kernel (split-precision bf16x3, split-K) against fp64 numpy, through the C ABI."""
+"""wgmma dense kernel (split-precision bf16x3, split-K) against fp64 numpy, through the C ABI."""
 import ctypes as C
 
 import numpy as np
@@ -43,8 +43,8 @@ def run_dense(model, rows, K, n_out, act, splits, seed=0):
     (64, 1024, 10000, 0, 0),   # vocabulary GEMM: partial last tile
     (64, 1024, 512, 1, 0),     # attend fc_1b + tanh
     (3, 72, 50, 1, 1),         # ragged K (zero padded k-block) and ragged n_out
-    (200, 512, 512, 1, 1),     # N = 208 activation rows
-    (384, 2048, 1024, 1, 0),   # two activation-row tiles (beam-search batch)
+    (200, 512, 512, 1, 1),     # two activation-row tiles of N = 112
+    (384, 2048, 1024, 1, 0),   # three activation-row tiles (beam-search batch)
     (784, 512, 512, 1, 1),     # context projection (4 images x 196 locations)
 ])
 def test_dense_umma_matches_fp64(model, rows, K, n_out, act, splits):

@@ -133,7 +133,7 @@ def test_one_pass_prologue_matches_the_three_launch_prologue(B):
 def test_packed_activation_and_prepass_paths_agree():
     """Operands packed by their producer kernels (default) vs the cooperative pre-pass vs per-stage producer
     warps: the same bf16 hi/lo split feeds the same MMAs.  The two conversion paths agree bit for bit; the packed path
-    sums even and odd K blocks in two TMEM accumulators (two MMA warps), so it agrees with them to fp32 round-off."""
+    issues the same MMAs in the same order, so it agrees with them to fp32 round-off."""
     ocfg, w, m = make_pair(4)
     ctx = R.synth_contexts(ocfg, 4)
     toks = {}
@@ -302,7 +302,7 @@ def test_chained_launch_agrees_with_the_per_layer_launches(shape):
 
 
 def test_config3_as_stated():
-    """BASELINE config 3 exactly as stated: B=256, L=196, D=2048, H=1536, V=10000 — the att_fused_kernel grid of 148 CTAs
+    """BASELINE config 3 exactly as stated: B=256, L=196, D=2048, H=1536, V=10000 — the att_fused_kernel grid that fills the GPU
     with two row tiles per dense layer that bench.py --workload 3 times.  Three greedy steps, logits of each step."""
     ocfg, w, m = make_pair(256, num_ctx=196, dim_ctx=2048, num_lstm_units=1536, vocabulary_size=10000)
     ctx = R.synth_contexts(ocfg, 256)

@@ -59,7 +59,7 @@ TC_DIMS = dict(num_ctx=32, dim_ctx=128, dim_embedding=64, num_lstm_units=64, dim
 @pytest.mark.parametrize("seed", [0, 31])
 def test_tensor_core_attend_projection_in_training(seed):
     """Shapes at which attend/fc_1a (forward and weight gradient; dim_ctx, dim_attend_layer and B*L multiples of 128)
-    and every batch-row product (forward, and dx where the output width is a multiple of 64) run on the tcgen05 dense
+    and every batch-row product (forward, and dx where the output width is a multiple of 64) run on the wgmma dense
     kernel: same parity bars, and agreement with the CUDA-core path."""
     # B = 16, T = 4: T*B = 64 rows, so the weight gradients of the batch-row layers are also taken as ONE stacked
     # product per layer after the time loop
@@ -155,7 +155,7 @@ def test_reference_shapes_one_step():
 def test_config4_widths_every_gradient(seed):
     """BASELINE config 4 per-GPU shapes (B=64, L=196, D=512, H=1024, V=10000; T=4 keeps the fp64 autograd oracle to
     seconds): losses and EVERY gradient against the oracle at the widths bench.py --workload 4 times, dropout off
-    and with injected masks — the shapes at which every product of the step runs on the tcgen05 dense kernel
+    and with injected masks — the shapes at which every product of the step runs on the wgmma dense kernel
     (attend/fc_1a forward + weight gradient, the batch-row layers, the stacked weight gradients with T*B = 256 rows,
     the ragged K = V input gradient of the vocabulary layer)."""
     import warnings

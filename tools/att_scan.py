@@ -14,7 +14,7 @@ alpha = torch.empty(B, L, device="cuda"); z = torch.empty(B, D, device="cuda")
 flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda")
 m.prepare(ctx, want_state=False)
 p = lambda t: C.c_void_p(t.data_ptr())
-for occ, sms in ((8, 148), (16, 148), (8, 64), (16, 64)):
+for occ, sms in ((8, 132), (16, 132), (8, 64), (16, 64)):
     for cold in (True, False):
         m.set_option("att_warps", occ)
         m.set_option("att_sms", sms)

@@ -1,9 +1,9 @@
-// tools/stream_bench.cu — per-SM ingest rate of 1-D bulk TMA (cp.async.bulk global -> shared) on B200.
+// tools/stream_bench.cu — per-SM ingest rate of 1-D bulk TMA (cp.async.bulk global -> shared) on H100.
 // Each CTA streams `per_cta` bytes through a ring of `nslots` x `chunk` bytes with no compute (one lane issues, the same
 // lane waits and releases), from (a) an L2-resident region (every CTA re-reads a small window) or (b) HBM (disjoint
 // regions, buffer >> L2).  Answers: what is the most one SM can pull, and how does it scale with the number of SMs
 // pulling at once?  (The decode step's dense CTAs and attention CTAs all sit at ~55 GB/s per SM.)
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/stream_bench tools/stream_bench.cu && tools/stream_bench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/stream_bench tools/stream_bench.cu && tools/stream_bench
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -91,9 +91,9 @@ int main() {
     cudaMalloc(&buf, buf_bytes);
     cudaMemset(buf, 1, buf_bytes);
     unsigned long long* t;
-    cudaMalloc(&t, 2 * 148 * 8);
+    cudaMalloc(&t, 2 * 132 * 8);
     cudaFuncSetAttribute(stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    unsigned long long h[2 * 148];
+    unsigned long long h[2 * 132];
     printf("source,grid,chunk_KB,ring_KB,per_cta_MB,GBps_per_SM_mean,GBps_per_SM_min,aggregate_TBps\n");
     // (c) the dense layers' activation operand: the SAME L2-resident blocks fetched by many CTAs at once
     for (int share : {4, 32, 128})
@@ -127,14 +127,14 @@ int main() {
                        (double)nchunks * chunk * grid / (double)(b - a) / 1e3);
             }
     for (int hbm = 0; hbm < 2; ++hbm)
-        for (int grid : {1, 16, 64, 79, 128, 148})
+        for (int grid : {1, 16, 64, 79, 128, 132})
             for (int chunk : {16 * 1024, 32 * 1024, 48 * 1024})
                 for (int ring : {96 * 1024, 192 * 1024}) {
                     const int nslots = ring / chunk;
                     if (nslots < 2) continue;
                     const size_t per_cta = hbm ? (size_t)12 << 20 : (size_t)8 << 20;
                     const int nchunks = (int)(per_cta / chunk);
-                    // L2: every CTA cycles over its own 256 KB window (148 x 256 KB = 37 MB, resident after the warm-up
+                    // L2: every CTA cycles over its own 256 KB window (132 x 256 KB = 33 MB, resident after the warm-up
                     // run); HBM: disjoint 12 MB regions, and a 2 GB buffer swept between runs
                     const size_t region = hbm ? per_cta : (size_t)256 << 10;
                     const size_t stride = hbm ? per_cta : region;
