@@ -139,6 +139,26 @@ int sat_beam_search(sat_handle* h, const float* contexts, int32_t n_img, int32_t
                     int32_t eos_id, int32_t* sentences, int32_t* lengths, double* scores, int32_t* n_results,
                     int32_t* is_complete, void* stream);
 
+/* Per-word maps: where the model looked for each word and how probable each word was.  Either output may be NULL; a
+ * call that requests neither runs exactly what sat_decode_loop / sat_beam_search run.
+ * With the default 2-layer attend, alpha does not depend on the LSTM state in inference (model.py:417-436: the score
+ * is w2.tanh(fc_1a(ctx)) + w2.tanh(fc_1b(h)), and the second term, the same for every location, cancels in the
+ * softmax), so the map of an image is the same for every word, as in the reference; the 1-layer attend gives
+ * word-dependent maps.
+ *
+ * sat_decode_loop_maps: sat_decode_loop plus alphas [T,B,L] (the layout of logits_all; alphas[t] is the alpha of the word emitted at step t)
+ * and word_probs [B,T] = softmax(logits of step t)[w], w the word fed to step t+1: the argmax (greedy) or
+ * forced_words[b,t] (teacher forced; a forced word outside [0, V) gets probability 0).  A call with maps runs the
+ * default launch layouts (never the experimental "chain" = 1 launch). */
+int sat_decode_loop_maps(sat_handle* h, const float* contexts, int32_t B, int32_t T, const int32_t* forced_words,
+                         int32_t* tokens, float* logits_all, float* alphas, float* word_probs, void* stream);
+/* sat_beam_search_maps: sat_beam_search plus, for each returned caption (same order as sentences): alphas [n_img, beam, T, L] and
+ * word_probs [n_img, beam, T], zero past lengths[k, j]; scores[k, j] is the product of word_probs[k, j, :len] in
+ * step order (fp64).  The first call with maps allocates a history of max_caption_length x max_batch x L floats. */
+int sat_beam_search_maps(sat_handle* h, const float* contexts, int32_t n_img, int32_t beam_size, int32_t T,
+                         int32_t eos_id, int32_t* sentences, int32_t* lengths, double* scores, int32_t* n_results,
+                         int32_t* is_complete, float* alphas, float* word_probs, void* stream);
+
 /* host-buffer forms: copy in, run, copy out, synchronise (what a sess.run caller sees) */
 int sat_decode_step_host(sat_handle* h, const float* contexts_host, int32_t contexts_changed,
                          const int32_t* last_word_host, const float* last_memory_host,

@@ -82,3 +82,35 @@ def write_test_results(path, image_files, captions, scores):
         for i, (a, c, p) in enumerate(zip(image_files, captions, scores)):
             w.writerow([i, a, c, repr(float(p))])
     return path
+
+
+def write_attention_maps(path, image_files, captions, vocabulary):
+    """One .npz (readable with np.load(..., allow_pickle=False)) with, for image i and its caption `captions[i]` (a
+    CaptionData from beam_search(with_attention=True)):
+      image_files                       [n] str
+      img<i>_word_ids / img<i>_words    the caption's word ids and words, tokenised as Vocabulary.get_sentence does
+                                        (up to and including the first '.')
+      img<i>_score, img<i>_word_probs   the caption's score and the probability of each of those words
+      img<i>_alphas                     where the model looked for each word: [len, sqrt(L), sqrt(L)] when L is a
+                                        square (14 x 14 for VGG conv5_3, 7 x 7 for ResNet res5c), else [len, L]"""
+    import numpy as np
+    out = {"image_files": np.asarray([str(f) for f in image_files])}
+    for i, cd in enumerate(captions):
+        if cd.alphas is None or cd.word_probs is None:
+            raise ValueError("caption %d carries no maps: use beam_search(..., with_attention=True)" % i)
+        ids = [int(w) for w in cd.sentence]
+        if "." in (vocabulary.words[w] for w in ids):
+            ids = ids[:[vocabulary.words[w] for w in ids].index(".") + 1]
+        n = len(ids)
+        alphas = np.asarray(cd.alphas, np.float32)[:n]
+        L = alphas.shape[1]
+        side = int(round(L ** 0.5))
+        if side * side == L:
+            alphas = alphas.reshape(n, side, side)
+        out["img%d_word_ids" % i] = np.asarray(ids, np.int32)
+        out["img%d_words" % i] = np.asarray([vocabulary.words[w] for w in ids], dtype=str)
+        out["img%d_score" % i] = np.float64(cd.score)
+        out["img%d_word_probs" % i] = np.asarray(cd.word_probs, np.float32)[:n]
+        out["img%d_alphas" % i] = alphas
+    np.savez(path, **out)
+    return path

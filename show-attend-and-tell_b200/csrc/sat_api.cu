@@ -54,6 +54,9 @@ struct Layer {
     unsigned long long* am_key = nullptr;   // fused-argmax tile candidates
     unsigned* am_ctr = nullptr;
     size_t am_n = 0;
+    float* am_sum = nullptr;     // word probabilities: per-tile softmax partials (like am_key), forced-word logits
+    float* am_wlogit = nullptr;
+    size_t am_sum_n = 0;
 };
 
 struct VecParam {  // a kernel of shape [n,1] kept as a plain fp32 vector
@@ -101,6 +104,9 @@ struct sat_handle {
     float* topk_p = nullptr;
     double* part_score = nullptr;
     void* comp_heap = nullptr;
+    // beam maps (sat_beam_search_maps), allocated on the first request: back-pointer history, see BeamParams
+    float *hist_alpha = nullptr, *hist_p = nullptr, *comp_p = nullptr;
+    int32_t *hist_parent = nullptr, *comp_prov = nullptr, *res_src = nullptr;
     // host-form staging
     float* stage_ctx = nullptr;
     void* stage_misc = nullptr;
@@ -219,6 +225,8 @@ static void layer_free(Layer& ly) {
     cudaFree(ly.xbar);
     cudaFree(ly.am_key);
     cudaFree(ly.am_ctr);
+    cudaFree(ly.am_sum);
+    cudaFree(ly.am_wlogit);
     ly = Layer();
 }
 
@@ -264,7 +272,8 @@ extern "C" void sat_destroy(sat_handle* h) {
                     h->t_dec, h->logits, h->st_c[0], h->st_c[1], h->st_h[0], h->st_h[1], h->word, h->zero_word,
                     h->rowcnt, h->topk_idx, h->part_n, h->comp_n, h->comp_sent, h->sent[0], h->sent[1], h->topk_p,
                     h->part_score, h->comp_heap, h->stage_ctx, h->stage_misc, h->att_part, h->trace, h->pa_h[0], h->pa_h[1], h->pa_z, h->pa_emb, h->pa_t, h->pa_z2[1], h->z2[1],
-                    h->chain_ctr, h->chain_scratch, h->chain_best};
+                    h->chain_ctr, h->chain_scratch, h->chain_best, h->hist_alpha, h->hist_p, h->comp_p, h->hist_parent,
+                    h->comp_prov, h->res_src};
     for (void* b : bufs) cudaFree(b);
     delete h;
 }
@@ -992,9 +1001,23 @@ static int attach_argmax(sat_handle* h, Layer& ly, LinProblem& P, const RowsPara
             CK(cudaMemset(ly.am_ctr, 0, 2 * sizeof(unsigned)));
         }
     }
+    if (am->word_probs && ly.am_sum_n < ly.am_n) {   // (only handles that ask for word probabilities)
+        if (stream_capturing(st)) return fail(SAT_ERR_STATE, "%s: scratch growth during graph capture", ly.name.c_str());
+        CK(cudaDeviceSynchronize());
+        cudaFree(ly.am_sum);
+        cudaFree(ly.am_wlogit);
+        ly.am_sum = ly.am_wlogit = nullptr; ly.am_sum_n = 0;
+        RET(dmalloc(&ly.am_sum, ly.am_n));
+        RET(dmalloc(&ly.am_wlogit, (size_t)h->max_rows));
+        ly.am_sum_n = ly.am_n;
+    }
     P.am_key = ly.am_key; P.am_ctr = ly.am_ctr;
     P.am_tokens = am->tokens; P.am_tokens_ld = am->tokens_ld; P.am_step = am->step;
     P.am_next_word = am->next_word; P.am_forced = am->forced; P.am_forced_ld = am->forced_ld;
+    if (am->word_probs) {
+        P.am_probs = am->word_probs; P.am_probs_ld = am->tokens_ld;
+        P.am_sum = ly.am_sum; P.am_wlogit = ly.am_wlogit;
+    }
     return 1;
 }
 
@@ -1178,8 +1201,11 @@ static int run_graphed(sat_handle* h, const std::vector<long long>& key, cudaStr
 // Decode loop with the attention of step t+1 (needs only q(t+1) = f(h_t)) running CONCURRENTLY with the
 // vocabulary layer of step t (needs only t_dec(t)); they join before the LSTM of step t+1, which consumes the
 // context vector of the one and the chosen word of the other.
+// alphas [T,B,L] / word_probs [B,T] (may be null): the per-word maps of sat_decode_loop_maps
+static float* step_alpha(float* alphas, int t, int B, int L) { return alphas ? alphas + (size_t)t * B * L : nullptr; }
+
 static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, const int32_t* forced, int32_t* tokens,
-                                float* logits_all, cudaStream_t st) {
+                                float* logits_all, float* alphas, float* word_probs, cudaStream_t st) {
     if (!h->side) {
         CK(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
@@ -1197,7 +1223,7 @@ static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, c
         float* zcur = h->z2[t & 1];          // context vector of this step (fp32 + packed), written by attention(t)
         h->pa_cur_z = h->pa_z2[t & 1];
         if (t == 0)   // q(0), attention(0) and the embedding of <start>
-            RET(attention_impl(h, ctx, B, 1, h_in, nullptr, zcur, st, false, h->word));
+            RET(attention_impl(h, ctx, B, 1, h_in, step_alpha(alphas, 0, B, d.num_ctx), zcur, st, false, h->word));
         RET(lstm_impl(h, zcur, h->word, c_in, h_in, c_out, h_out, B, st));
         float* logits = logits_all ? logits_all + (size_t)t * B * d.vocabulary_size : h->logits;
         if (t + 1 < T) {
@@ -1215,7 +1241,8 @@ static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, c
             // the SMs left over
             int budget = h->opt_att_sms > 0 ? h->opt_att_sms : h->num_sms - h->dec_2.n_tiles;
             if (budget < h->num_sms / 4) budget = h->num_sms;
-            RET(attention_impl(h, ctx, B, 1, h_out, nullptr, h->z2[(t + 1) & 1], h->side, true, nullptr, budget));
+            RET(attention_impl(h, ctx, B, 1, h_out, step_alpha(alphas, t + 1, B, d.num_ctx), h->z2[(t + 1) & 1], h->side,
+                               true, nullptr, budget));
             CK(cudaEventRecord(h->ev_join, h->side));
             h->pa_cur_h_in = h->pa_h[t & 1];
             h->pa_cur_z = h->pa_z2[t & 1];
@@ -1224,7 +1251,7 @@ static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, c
         RowsParams rp;
         memset(&rp, 0, sizeof(rp));
         rp.tokens = tokens; rp.tokens_ld = T; rp.step = t;
-        rp.next_word = h->word; rp.forced = forced; rp.forced_ld = T;
+        rp.next_word = h->word; rp.forced = forced; rp.forced_ld = T; rp.word_probs = word_probs;
         int fused = 0;
         RET(decode_impl(h, h_out, zcur, h->word, logits, B, st, false, &rp, &fused, 2, t + 1 < T));  // fc_2 + argmax
         if (!fused) {
@@ -1245,7 +1272,7 @@ static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, c
 // grid leaves idle and the two run side by side without a second stream; it only waits for its predecessor
 // right before it exits, which keeps "kernel k complete => kernel k-1 complete" for the LSTM that follows.
 static int loop_enqueue_chain(sat_handle* h, const float* ctx, int B, int T, const int32_t* forced, int32_t* tokens,
-                              float* logits_all, cudaStream_t st, bool prepared = false) {
+                              float* logits_all, float* alphas, float* word_probs, cudaStream_t st, bool prepared = false) {
     const sat_dims& d = h->d;
     if (!prepared) RET(prepare_impl(h, ctx, B, h->st_c[0], h->st_h[0], st, h->pa_h[0]));
     CK(cudaMemsetAsync(h->word, 0, (size_t)B * sizeof(int32_t), st));  // <start> = 0 (model.py:254)
@@ -1259,14 +1286,14 @@ static int loop_enqueue_chain(sat_handle* h, const float* ctx, int B, int T, con
         h->pa_cur_h_out = h->pa_h[(t + 1) & 1];
         h->pa_cur_z = h->pa_z;
         if (t == 0)   // q(0), attention(0) and the embedding of <start>
-            RET(attention_impl(h, ctx, B, 1, h_in, nullptr, h->z, st, false, h->word));
+            RET(attention_impl(h, ctx, B, 1, h_in, step_alpha(alphas, 0, B, d.num_ctx), h->z, st, false, h->word));
         RET(lstm_impl(h, h->z, h->word, c_in, h_in, c_out, h_out, B, st));
         float* logits = logits_all ? logits_all + (size_t)t * B * d.vocabulary_size : h->logits;
         RET(decode_impl(h, h_out, h->z, h->word, logits, B, st, t + 1 < T, nullptr, nullptr, 1));   // fc_1 || q(t+1)
         RowsParams rp;
         memset(&rp, 0, sizeof(rp));
         rp.tokens = tokens; rp.tokens_ld = T; rp.step = t;
-        rp.next_word = h->word; rp.forced = forced; rp.forced_ld = T;
+        rp.next_word = h->word; rp.forced = forced; rp.forced_ld = T; rp.word_probs = word_probs;
         int fused = 0;
         RET(decode_impl(h, h_out, h->z, h->word, logits, B, st, false, &rp, &fused, 2, t + 1 < T));  // fc_2 + argmax
         if (!fused) {
@@ -1275,7 +1302,8 @@ static int loop_enqueue_chain(sat_handle* h, const float* ctx, int B, int T, con
         }
         if (t + 1 < T) {
             h->pa_cur_h_in = h->pa_h[(t + 1) & 1];
-            RET(attention_impl(h, ctx, B, 1, h_out, nullptr, h->z, st, true, nullptr, budget, true));
+            RET(attention_impl(h, ctx, B, 1, h_out, step_alpha(alphas, t + 1, B, d.num_ctx), h->z, st, true, nullptr, budget,
+                               true));
         }
     }
     h->pa_on = false;
@@ -1456,14 +1484,15 @@ static bool vocab_argmax_fits(sat_handle* h, int B) {
 }
 
 static int loop_enqueue(sat_handle* h, const float* ctx, int B, int T, const int32_t* forced, int32_t* tokens,
-                        float* logits_all, cudaStream_t st) {
+                        float* logits_all, float* alphas, float* word_probs, cudaStream_t st) {
     const bool pa = h->pa_ok && h->opt_pa && h->opt_gemm != 0;
     const bool am = pa && vocab_argmax_fits(h, B);
-    if (fused_loop_available(h, B)) return loop_enqueue_fused(h, ctx, B, T, forced, tokens, logits_all, st, false);
+    const bool maps = alphas || word_probs;   // (the experimental chained launch takes no maps)
+    if (!maps && fused_loop_available(h, B)) return loop_enqueue_fused(h, ctx, B, T, forced, tokens, logits_all, st, false);
     if (am && h->opt_overlap == 2 && h->opt_pdl && h->d.num_decode_layers == 2)
-        return loop_enqueue_chain(h, ctx, B, T, forced, tokens, logits_all, st);
+        return loop_enqueue_chain(h, ctx, B, T, forced, tokens, logits_all, alphas, word_probs, st);
     if (am && h->opt_overlap && h->d.num_decode_layers == 2 && st != nullptr && st != cudaStreamLegacy)
-        return loop_enqueue_overlap(h, ctx, B, T, forced, tokens, logits_all, st);
+        return loop_enqueue_overlap(h, ctx, B, T, forced, tokens, logits_all, alphas, word_probs, st);
     RET(prepare_impl(h, ctx, B, h->st_c[0], h->st_h[0], st, pa ? h->pa_h[0] : nullptr));
     CK(cudaMemsetAsync(h->word, 0, (size_t)B * sizeof(int32_t), st));  // <start> = 0 (model.py:254)
     bool emb_valid = false;
@@ -1474,9 +1503,11 @@ static int loop_enqueue(sat_handle* h, const float* ctx, int B, int T, const int
         io.c_in = h->st_c[t & 1]; io.h_in = h->st_h[t & 1];
         io.c_out = h->st_c[(t + 1) & 1]; io.h_out = h->st_h[(t + 1) & 1];
         io.logits = logits_all ? logits_all + (size_t)t * B * h->d.vocabulary_size : nullptr;
+        io.alpha = step_alpha(alphas, t, B, h->d.num_ctx);
         io.want_rows = true;
         io.rows.tokens = tokens; io.rows.tokens_ld = T; io.rows.step = t;
         io.rows.next_word = h->word; io.rows.forced = forced; io.rows.forced_ld = T;
+        io.rows.word_probs = word_probs;
         io.q_ready = t > 0;
         io.make_next_q = t + 1 < T;
         io.pa_slot = t & 1;          // initialize / the previous LSTM wrote the packed h into this slot
@@ -1500,7 +1531,7 @@ static bool chain_loop_available(sat_handle* h, int B) {
 // (may be null) is an event the contexts depend on; with a null event the CALLER guarantees that the contexts are
 // complete when the call is made (they must not be produced by earlier work queued on `st`).
 static int decode_loop_xbatch(sat_handle* h, const float* contexts, int B, int T, const int32_t* forced, int32_t* tokens,
-                              float* logits_all, cudaStream_t st, cudaEvent_t input_ready) {
+                              float* logits_all, float* alphas, float* word_probs, cudaStream_t st, cudaEvent_t input_ready) {
     const sat_dims& d = h->d;
     if (!h->xb_stream) {
         CK(cudaStreamCreateWithFlags(&h->xb_stream, cudaStreamNonBlocking));
@@ -1533,7 +1564,7 @@ static int decode_loop_xbatch(sat_handle* h, const float* contexts, int B, int T
     float *T1_keep = h->T1, *c_keep = h->st_c[0], *h_keep = h->st_h[0];
     uint8_t* pa_keep = h->pa_h[0];
     h->T1 = S.T1; h->st_c[0] = S.c0; h->st_h[0] = S.h0; h->pa_h[0] = S.pa_h0;
-    int rc = run_graphed(h, {3, (long long)contexts, B, slot}, h->xb_stream, [&]() -> int {
+    int rc = run_graphed(h, {3, (long long)contexts, B, slot, (long long)alphas, (long long)word_probs}, h->xb_stream, [&]() -> int {
         return prepare_impl(h, contexts, B, h->st_c[0], h->st_h[0], h->xb_stream, h->pa_h[0]);
     });
     if (rc == SAT_OK) {
@@ -1541,10 +1572,12 @@ static int decode_loop_xbatch(sat_handle* h, const float* contexts, int B, int T
         cudaStreamWaitEvent(st, S.ev_prep, 0);
         h->prep_ctx = contexts;
         h->prep_ni = B;
-        rc = run_graphed(h, {4, (long long)contexts, B, T, (long long)forced, (long long)tokens, (long long)logits_all, slot}, st,
+        rc = run_graphed(h, {4, (long long)contexts, B, T, (long long)forced, (long long)tokens, (long long)logits_all, slot,
+                             (long long)alphas, (long long)word_probs}, st,
                          [&]() -> int {
-                             return fused_loop_available(h, B) ? loop_enqueue_fused(h, contexts, B, T, forced, tokens, logits_all, st, true)
-                                                               : loop_enqueue_chain(h, contexts, B, T, forced, tokens, logits_all, st, true);
+                             return (fused_loop_available(h, B) && !alphas && !word_probs)
+                                        ? loop_enqueue_fused(h, contexts, B, T, forced, tokens, logits_all, st, true)
+                                        : loop_enqueue_chain(h, contexts, B, T, forced, tokens, logits_all, alphas, word_probs, st, true);
                          });
         cudaEventRecord(S.ev_done, st);
         S.used = true;
@@ -1556,17 +1589,23 @@ static int decode_loop_xbatch(sat_handle* h, const float* contexts, int B, int T
 
 extern "C" int sat_decode_loop(sat_handle* h, const float* contexts, int32_t B, int32_t T, const int32_t* forced_words,
                                int32_t* tokens, float* logits_all, void* stream) {
+    return sat_decode_loop_maps(h, contexts, B, T, forced_words, tokens, logits_all, nullptr, nullptr, stream);
+}
+
+extern "C" int sat_decode_loop_maps(sat_handle* h, const float* contexts, int32_t B, int32_t T, const int32_t* forced_words,
+                                    int32_t* tokens, float* logits_all, float* alphas, float* word_probs, void* stream) {
     RET(require_ready(h));
     if (!contexts || !tokens) return fail(SAT_ERR_INVALID, "sat_decode_loop: null tensor");
     if (B < 1 || B > h->max_rows) return fail(SAT_ERR_INVALID, "batch %d outside [1, %d]", B, h->max_rows);
     if (T < 1) return fail(SAT_ERR_INVALID, "T must be >= 1");
     cudaStream_t st = (cudaStream_t)stream;
     if (h->opt_xbatch && chain_loop_available(h, B) && st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread)
-        return decode_loop_xbatch(h, contexts, B, T, forced_words, tokens, logits_all, st, nullptr);
+        return decode_loop_xbatch(h, contexts, B, T, forced_words, tokens, logits_all, alphas, word_probs, st, nullptr);
+    // the map buffers are part of the key: a replayed graph writes into the buffers it was captured with
     std::vector<long long> key = {1, (long long)contexts, B, T, (long long)forced_words, (long long)tokens,
-                                  (long long)logits_all};
+                                  (long long)logits_all, (long long)alphas, (long long)word_probs};
     const int rc = run_graphed(h, key, st, [&]() -> int {
-        return loop_enqueue(h, contexts, B, T, forced_words, tokens, logits_all, st);
+        return loop_enqueue(h, contexts, B, T, forced_words, tokens, logits_all, alphas, word_probs, st);
     });
     // A replayed graph re-projects `contexts` into T1 on the device without passing through prepare_impl: the host-side
     // record of what T1 holds must follow in every case (eager, capture, replay), or a later single step on other
@@ -1577,7 +1616,9 @@ extern "C" int sat_decode_loop(sat_handle* h, const float* contexts, int32_t B, 
 
 // ------------------------------------------------------------ beam search
 static int beam_enqueue(sat_handle* h, const float* ctx, int NI, int beam, int T, int eos, int32_t* sentences,
-                        int32_t* lengths, double* scores, int32_t* n_results, int32_t* is_complete, cudaStream_t st) {
+                        int32_t* lengths, double* scores, int32_t* n_results, int32_t* is_complete, float* alphas,
+                        float* word_probs, cudaStream_t st) {
+    const bool maps = alphas || word_probs;
     const sat_dims& d = h->d;
     const int H = d.num_lstm_units;
     // states: st_*[0] = inputs of the current step, st_*[1] = outputs
@@ -1594,11 +1635,18 @@ static int beam_enqueue(sat_handle* h, const float* ctx, int NI, int beam, int T
     bp.next_word = h->word;
     bp.res_sent = sentences; bp.res_len = lengths; bp.res_score = scores; bp.res_n = n_results;
     bp.res_complete = is_complete;
+    const size_t NB = (size_t)NI * beam;
+    if (maps) {
+        bp.hist_alpha = h->hist_alpha; bp.hist_parent = h->hist_parent; bp.hist_p = h->hist_p;
+        bp.comp_prov = h->comp_prov; bp.comp_p = h->comp_p; bp.res_src = h->res_src;
+        bp.L = d.num_ctx; bp.res_alpha = alphas; bp.res_probs = word_probs;
+    }
     for (int idx = 0; idx < T; ++idx) {                                       // base_model.py:184
         const int G = idx == 0 ? 1 : beam;                                    // base_model.py:191
         StepIO io;
         memset(&io, 0, sizeof(io));
         io.ctx = ctx; io.n_img = NI; io.group = G;
+        if (maps) io.alpha = h->hist_alpha + (size_t)idx * NB * d.num_ctx;   // rows img*G + g
         io.last_word = idx == 0 ? h->zero_word : h->word;                     // base_model.py:193-198
         io.c_in = h->st_c[0]; io.h_in = h->st_h[0]; io.c_out = h->st_c[1]; io.h_out = h->st_h[1];
         io.want_rows = true;
@@ -1614,12 +1662,24 @@ static int beam_enqueue(sat_handle* h, const float* ctx, int NI, int beam, int T
     bp.step = T;
     CK(beam_finalize_launch(bp, st));
     h->launches += 1;
+    if (maps) {
+        CK(beam_maps_launch(bp, st));
+        h->launches += 1;
+    }
     return SAT_OK;
 }
 
 extern "C" int sat_beam_search(sat_handle* h, const float* contexts, int32_t n_img, int32_t beam_size, int32_t T,
                                int32_t eos_id, int32_t* sentences, int32_t* lengths, double* scores,
                                int32_t* n_results, int32_t* is_complete, void* stream) {
+    return sat_beam_search_maps(h, contexts, n_img, beam_size, T, eos_id, sentences, lengths, scores, n_results,
+                                is_complete, nullptr, nullptr, stream);
+}
+
+extern "C" int sat_beam_search_maps(sat_handle* h, const float* contexts, int32_t n_img, int32_t beam_size, int32_t T,
+                                    int32_t eos_id, int32_t* sentences, int32_t* lengths, double* scores,
+                                    int32_t* n_results, int32_t* is_complete, float* alphas, float* word_probs,
+                                    void* stream) {
     RET(require_ready(h));
     if (!contexts || !sentences || !lengths || !scores || !n_results || !is_complete)
         return fail(SAT_ERR_INVALID, "sat_beam_search: null tensor");
@@ -1629,11 +1689,23 @@ extern "C" int sat_beam_search(sat_handle* h, const float* contexts, int32_t n_i
         return fail(SAT_ERR_INVALID, "n_img*beam %lld > max_batch %d", (long long)n_img * beam_size, h->max_rows);
     if (h->d.vocabulary_size < beam_size + 2) return fail(SAT_ERR_INVALID, "vocabulary too small for beam %d", beam_size);
     cudaStream_t st = (cudaStream_t)stream;
+    if ((alphas || word_probs) && !h->hist_alpha) {   // history of the first request, sized for the handle's limits
+        if (T > 1024) return fail(SAT_ERR_UNSUPPORTED, "beam maps: T %d > 1024", T);
+        if (stream_capturing(st)) return fail(SAT_ERR_STATE, "beam maps: allocation during graph capture");
+        const size_t R = (size_t)h->max_rows, TM = (size_t)h->d.max_caption_length;
+        RET(dmalloc(&h->hist_alpha, TM * R * h->d.num_ctx));
+        RET(dmalloc(&h->hist_parent, TM * R));
+        RET(dmalloc(&h->hist_p, TM * R));
+        RET(dmalloc(&h->comp_prov, R));
+        RET(dmalloc(&h->comp_p, R));
+        RET(dmalloc(&h->res_src, R));
+    }
     std::vector<long long> key = {2, (long long)contexts, n_img, beam_size, T, eos_id, (long long)sentences,
-                                  (long long)lengths, (long long)scores, (long long)n_results, (long long)is_complete};
+                                  (long long)lengths, (long long)scores, (long long)n_results, (long long)is_complete,
+                                  (long long)alphas, (long long)word_probs};
     const int rc = run_graphed(h, key, st, [&]() -> int {
         return beam_enqueue(h, contexts, n_img, beam_size, T, eos_id, sentences, lengths, scores, n_results,
-                            is_complete, st);
+                            is_complete, alphas, word_probs, st);
     });
     note_projected(h, rc == SAT_OK ? contexts : nullptr, n_img);   // (see sat_decode_loop)
     return rc;
@@ -1751,7 +1823,7 @@ extern "C" int sat_decode_loop_host_submit(sat_handle* h, const float* contexts_
     CK(cudaEventRecord(h->pipe_up[slot], h->pipe_copy));
     CK(cudaStreamWaitEvent(st, h->pipe_up[slot], 0));      // (forced words; and the contexts when not overlapped)
     if (chain_loop_available(h, B) && st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread)
-        RET(decode_loop_xbatch(h, h->pipe_ctx[slot], B, T, forced, tok, nullptr, st, h->pipe_up[slot]));
+        RET(decode_loop_xbatch(h, h->pipe_ctx[slot], B, T, forced, tok, nullptr, nullptr, nullptr, st, h->pipe_up[slot]));
     else
         RET(sat_decode_loop(h, h->pipe_ctx[slot], B, T, forced, tok, nullptr, stream));
     CK(cudaMemcpyAsync(tokens_host, tok, TB * sizeof(int32_t), cudaMemcpyDeviceToHost, st));

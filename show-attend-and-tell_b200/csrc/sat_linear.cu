@@ -86,7 +86,9 @@ struct XChunk {
 };
 
 // NT = (row tile of the launch) / 16: the accumulator fragments per warpgroup
-template <int NT>
+// WP: the fused arg-max also produces the probability of the word fed to the next step (LinProblem::am_probs); a
+// separate instance, so that launches without it run the code they ran before
+template <int NT, bool WP>
 __global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_constant__ LinLaunch L) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // control block: barriers etc. live in the first 1024 bytes
@@ -579,6 +581,35 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_co
                     key = max(key, __shfl_xor_sync(0xffffffffu, key, 1));
                     key = max(key, __shfl_xor_sync(0xffffffffu, key, 2));
                     if (live && part == 0 && !dry) am_key[r] = key;
+                    if constexpr (WP) {
+                        // softmax partial of the row over this tile, relative to the tile maximum (the key's value)
+                        const float mt = argmax_key_value(key);
+                        float s = 0.f;
+#pragma unroll 2
+                        for (int j = 0; j < 8; ++j) {
+                            const int jj = (j + pt) & 7;
+                            const float4 a4 = row_t[jj];
+                            const int i0 = n_tile * kTileN + part * 32 + jj * 4;
+                            if (i0 + 0 < n_out) s += expf(a4.x - mt);
+                            if (i0 + 1 < n_out) s += expf(a4.y - mt);
+                            if (i0 + 2 < n_out) s += expf(a4.z - mt);
+                            if (i0 + 3 < n_out) s += expf(a4.w - mt);
+                        }
+                        s += __shfl_xor_sync(0xffffffffu, s, 1);
+                        s += __shfl_xor_sync(0xffffffffu, s, 2);
+                        if (live && part == 0) {
+                            float* const am_sum = P.am_sum + (size_t)(rt * P.n_tiles + n_tile) * N;
+                            if (!dry) am_sum[r] = s;
+                            if (P.am_forced) {   // teacher forcing: the tile that owns the forced word keeps its logit
+                                const int w = P.am_forced[(size_t)(row0 + r) * P.am_forced_ld + P.am_step];
+                                const int c = w - n_tile * kTileN;
+                                if (c >= 0 && c < kTileN && w < n_out) {
+                                    const float lw = row_base[r * row_mul + c];
+                                    if (!dry) P.am_wlogit[row0 + r] = lw;
+                                }
+                            }
+                        }
+                    }
                 }
             }
             if (splits > 1 && !dry) cluster_arrive_relaxed();   // this CTA no longer reads its peers' tiles
@@ -617,16 +648,39 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_co
                     const int rt2 = r / N, cc = r - rt2 * N;
                     const unsigned long long* pk = P.am_key + (size_t)rt2 * n_tiles * N + cc;
                     unsigned long long best = 0ull;
-                    for (int tl = pt; tl < n_tiles; tl += kLinProducers) best = max(best, __ldcg(pk + (size_t)tl * N));
+                    float lm = -INFINITY, ls = 0.f;   // (WP) merged softmax partials of this thread's tiles
+                    for (int tl = pt; tl < n_tiles; tl += kLinProducers) {
+                        const unsigned long long k = __ldcg(pk + (size_t)tl * N);
+                        best = max(best, k);
+                        if constexpr (WP) lse_merge(lm, ls, argmax_key_value(k), __ldcg(P.am_sum + (pk - P.am_key) + (size_t)tl * N));
+                    }
 #pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
-                    if ((pt & 31) == 0) red_s[pt >> 5] = best;
+                    for (int o = 16; o > 0; o >>= 1) {
+                        best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
+                        if constexpr (WP) lse_merge(lm, ls, __shfl_xor_sync(0xffffffffu, lm, o), __shfl_xor_sync(0xffffffffu, ls, o));
+                    }
+                    float2* const red_ms = reinterpret_cast<float2*>(smem_raw + 384);   // [8] (between red_s and the scratch line)
+                    if ((pt & 31) == 0) {
+                        red_s[pt >> 5] = best;
+                        if constexpr (WP) red_ms[pt >> 5] = make_float2(lm, ls);
+                    }
                     named_bar_sync(1, kLinProducers);
                     if (pt == 0) {
 #pragma unroll
-                        for (int w = 1; w < kLinProducers / 32; ++w) best = max(best, red_s[w]);
+                        for (int w = 1; w < kLinProducers / 32; ++w) {
+                            best = max(best, red_s[w]);
+                            if constexpr (WP) lse_merge(lm, ls, red_ms[w].x, red_ms[w].y);
+                        }
                         const int bi2 = argmax_key_index(best);
                         const int nw = P.am_forced ? P.am_forced[(size_t)r * P.am_forced_ld + P.am_step] : bi2;
+                        if constexpr (WP) {
+                            // softmax(logits)[nw] = exp(l_nw - M) / S; M is the row maximum (lm == its value); a forced
+                            // word outside [0, V) has probability 0 and is never used as an index
+                            float pw = 0.f;
+                            if (!P.am_forced) pw = 1.0f / ls;
+                            else if (nw >= 0 && nw < P.n_out) pw = expf(__ldcg(P.am_wlogit + r) - lm) / ls;
+                            if (!dry) P.am_probs[(size_t)r * P.am_probs_ld + P.am_step] = pw;
+                        }
                         if (!dry) {
                             if (P.am_tokens) P.am_tokens[(size_t)r * P.am_tokens_ld + P.am_step] = bi2;
                             if (P.am_next_word) P.am_next_word[r] = nw;
@@ -879,9 +933,11 @@ int device_sm_count() {
 
 static int g_smem_optin = 0;
 
-static void (*const g_lin_kernels[kMaxRowTile / 16])(LinLaunch) = {
-    lin_mma_kernel<1>, lin_mma_kernel<2>, lin_mma_kernel<3>, lin_mma_kernel<4>,
-    lin_mma_kernel<5>, lin_mma_kernel<6>, lin_mma_kernel<7>, lin_mma_kernel<8>};
+static void (*const g_lin_kernels[2][kMaxRowTile / 16])(LinLaunch) = {
+    {lin_mma_kernel<1, false>, lin_mma_kernel<2, false>, lin_mma_kernel<3, false>, lin_mma_kernel<4, false>,
+     lin_mma_kernel<5, false>, lin_mma_kernel<6, false>, lin_mma_kernel<7, false>, lin_mma_kernel<8, false>},
+    {lin_mma_kernel<1, true>, lin_mma_kernel<2, true>, lin_mma_kernel<3, true>, lin_mma_kernel<4, true>,
+     lin_mma_kernel<5, true>, lin_mma_kernel<6, true>, lin_mma_kernel<7, true>, lin_mma_kernel<8, true>}};
 
 cudaError_t lin_init_attrs() {
     int dev = 0;
@@ -889,10 +945,11 @@ cudaError_t lin_init_attrs() {
     if (e != cudaSuccess) return e;
     e = cudaDeviceGetAttribute(&g_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     if (e != cudaSuccess) return e;
-    for (auto k : g_lin_kernels) {
-        e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin);
-        if (e != cudaSuccess) return e;
-    }
+    for (auto& inst : g_lin_kernels)
+        for (auto k : inst) {
+            e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, g_smem_optin);
+            if (e != cudaSuccess) return e;
+        }
     return cudaSuccess;
 }
 
@@ -920,9 +977,14 @@ cudaError_t lin_launch(const LinLaunch& L, cudaStream_t st, bool use_simt) {
         lin_simt_kernel<<<total, 128, 0, st>>>(M);
         return cudaGetLastError();
     }
-    int max_rt = 16;
+    int max_rt = 16, wp = 0;
     for (int i = 0; i < L.nprob; ++i) {
         total += L.p[i].cta_count;
+        if (L.p[i].am_probs) {
+            if (!L.p[i].am_key || !L.p[i].am_sum || L.p[i].splits != 1 || (L.p[i].am_forced && !L.p[i].am_wlogit))
+                return cudaErrorInvalidValue;
+            wp = 1;
+        }
         if (L.p[i].row_tile > max_rt) max_rt = L.p[i].row_tile;
         // (one MMA width per launch: grouped problems share the row tile, so no MMA reads past its operand)
         if (L.p[i].row_tile % 16 || L.p[i].row_tile > kMaxRowTile || L.p[i].row_tile != L.p[0].row_tile)
@@ -959,7 +1021,7 @@ cudaError_t lin_launch(const LinLaunch& L, cudaStream_t st, bool use_simt) {
     }
     cfg.attrs = at;
     cfg.numAttrs = na;
-    return cudaLaunchKernelEx(&cfg, g_lin_kernels[max_rt / 16 - 1], L);
+    return cudaLaunchKernelEx(&cfg, g_lin_kernels[wp][max_rt / 16 - 1], L);
 }
 
 cudaError_t lin_repack_weight(const float* w_tf, int K, int n_out, int perm_H, uint8_t* wpack, int layout_mode,

@@ -75,7 +75,14 @@ struct LinProblem {
     int32_t* am_next_word; // [rows] or null
     const int32_t* am_forced;  // teacher-forced next words [rows, am_forced_ld] or null
     int am_forced_ld;
-    uint8_t* out_pa;       // optional packed copy of the output for the next dense layer (width n_out)
+    // optional probability of the word fed to the next step, softmax(logits)[w] (w = forced word or the arg-max),
+    // from per-tile partials (tile maximum = value half of the key, sum of exp(v - max)) merged online.  Needs the
+    // word-probability instance of the kernel (lin_launch picks it when am_probs is set).
+    float* am_probs;       // [rows, am_probs_ld] or null
+    int am_probs_ld;
+    float* am_sum;         // laid out like am_key: sum over the tile row of exp(v - tile maximum)
+    float* am_wlogit;      // [rows] teacher forcing: logit of the forced word, stored by the tile that owns it
+    uint8_t* out_pa;      // optional packed copy of the output for the next dense layer (width n_out)
     // fused epilogue of the vocabulary layer in loops: pack the embedding row of the chosen next word
     const float* am_emb;   // [V, E] embedding matrix or null
     int am_E;
@@ -145,6 +152,17 @@ __device__ __forceinline__ unsigned long long argmax_key(float v, int idx) {
     return ((unsigned long long)ord << 32) | (unsigned long long)(0xffffffffu - (unsigned)idx);
 }
 __device__ __forceinline__ int argmax_key_index(unsigned long long key) { return (int)(0xffffffffu - (unsigned)(key & 0xffffffffull)); }
+__device__ __forceinline__ float argmax_key_value(unsigned long long key) {
+    const unsigned ord = (unsigned)(key >> 32);
+    return __uint_as_float((ord & 0x80000000u) ? (ord & 0x7fffffffu) : ~ord);
+}
+// online-softmax merge of (max, sum of exp(v - max)) pairs; (-inf, 0) is the empty pair
+__device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2) {
+    const float M = fmaxf(m, m2);
+    if (M == -INFINITY) return;
+    s = s * expf(m - M) + s2 * expf(m2 - M);
+    m = M;
+}
 #endif
 
 constexpr int kAmSmemWords = 1024;   // rows whose chosen word the last CTA keeps in shared memory

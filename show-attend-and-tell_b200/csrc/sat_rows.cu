@@ -86,7 +86,7 @@ __global__ void __launch_bounds__(kRowThreads) rows_softmax_kernel(const RowsPar
         if (p.tokens) p.tokens[(size_t)row * p.tokens_ld + p.step] = best.i;
         if (p.next_word) p.next_word[row] = p.forced ? p.forced[(size_t)row * p.forced_ld + p.step] : best.i;
     }
-    if (!p.probs && p.topk == 0) return;  // greedy / teacher-forced loops only need the argmax
+    if (!p.probs && p.topk == 0 && !p.word_probs) return;  // greedy / teacher-forced loops only need the argmax
 
     float s = 0.f;
     if (CACHED) {
@@ -100,6 +100,13 @@ __global__ void __launch_bounds__(kRowThreads) rows_softmax_kernel(const RowsPar
     }
     s = block_sum(s, sm_f);
     const float inv = 1.0f / s;
+    if (p.word_probs) {
+        if (threadIdx.x == 0) {
+            const int w = p.forced ? p.forced[(size_t)row * p.forced_ld + p.step] : best.i;
+            p.word_probs[(size_t)row * p.tokens_ld + p.step] = (w >= 0 && w < V) ? expf(x[w] - m) * inv : 0.f;
+        }
+        if (!p.probs && p.topk == 0) return;
+    }
 
     // probabilities + thread-local top-kMaxTopK, kept sorted by (prob desc, index asc) with a compare-and-swap
     // chain on registers (static indices only)
@@ -176,7 +183,7 @@ cudaError_t rows_softmax_launch(const RowsParams& p, int rows, cudaStream_t st) 
 // ------------------------------------------------------------------ beam search
 // Python heapq semantics (CPython Lib/heapq.py) on tiny arrays, so that ties are
 // broken exactly as utils/misc.py:62-87 (TopN) does.
-struct PItem { double score; int parent; int word; };
+struct PItem { double score; int parent; int word; float p; };
 struct CItem { double score; int slot; int len; };
 
 template <typename T>
@@ -249,14 +256,18 @@ __global__ void __launch_bounds__(256) beam_update_kernel(const BeamParams p) {
                         int* dst = p.comp_sent + ((size_t)img * beam + slot) * T;
                         for (int t = 0; t < idx; ++t) dst[t] = sent_cur[(size_t)b * T + t];
                         dst[idx] = w;
+                        if (p.comp_prov) {   // (the step is len - 1 of the slot's CItem)
+                            p.comp_prov[(size_t)img * beam + slot] = b;
+                            p.comp_p[(size_t)img * beam + slot] = s_p[b * K + j];
+                        }
                     }
                 } else {                                                               // base_model.py:231-232
                     if (np < beam) {
-                        newp[np].score = sc; newp[np].parent = b; newp[np].word = w;
+                        newp[np].score = sc; newp[np].parent = b; newp[np].word = w; newp[np].p = s_p[b * K + j];
                         ++np;
                         heap_siftdown(newp, 0, np - 1);
                     } else if (newp[0].score < sc) {
-                        newp[0].score = sc; newp[0].parent = b; newp[0].word = w;
+                        newp[0].score = sc; newp[0].parent = b; newp[0].word = w; newp[0].p = s_p[b * K + j];
                         heap_siftup(newp, np, 0);
                     }
                 }
@@ -277,6 +288,11 @@ __global__ void __launch_bounds__(256) beam_update_kernel(const BeamParams p) {
     if ((int)threadIdx.x < np) {
         sent_next[(size_t)threadIdx.x * T + idx] = newp[threadIdx.x].word;
         p.next_word[(size_t)img * beam + threadIdx.x] = newp[threadIdx.x].word;
+        if (p.hist_parent) {
+            const size_t hi = (size_t)idx * p.NI * beam + (size_t)img * beam + threadIdx.x;
+            p.hist_parent[hi] = newp[threadIdx.x].parent;
+            p.hist_p[hi] = newp[threadIdx.x].p;
+        }
     }
     const int H4 = p.H >> 2;   // H % 32 == 0 (sat_create)
     for (int u = threadIdx.x; u < np * H4; u += blockDim.x) {
@@ -329,14 +345,62 @@ __global__ void beam_finalize_kernel(const BeamParams p) {
             for (int t = 0; t < T; ++t) dst[t] = t < len ? src[t] : -1;
             p.res_len[(size_t)img * beam + j] = len;
             p.res_score[(size_t)img * beam + j] = sc[j];
+            if (p.res_src) p.res_src[(size_t)img * beam + j] = use_comp ? p.comp_heap[(size_t)img * beam + o].slot : o;
         } else {
             for (int t = 0; t < T; ++t) dst[t] = -1;
             p.res_len[(size_t)img * beam + j] = 0;
             p.res_score[(size_t)img * beam + j] = 0.0;
+            if (p.res_src) p.res_src[(size_t)img * beam + j] = -1;
         }
     }
     p.res_n[img] = n;
     p.res_complete[img] = use_comp ? 1 : 0;
+}
+
+// Per-word maps of result (img, j): walk the caption back from its last word through the back-pointers
+//   word t of survivor j of step t came from live row r_t = hist_parent[t][j]; the survivor of step t-1 is j = r_t
+// and gather alpha rows and probabilities, zero past the caption's length.  One block per result.
+__global__ void __launch_bounds__(256) beam_maps_kernel(const BeamParams p) {
+    extern __shared__ int rows_s[];   // [T] live row of step t (row index inside the image's group)
+    __shared__ float p_s[1024];
+    const int res = blockIdx.x, img = res / p.beam;
+    const int beam = p.beam, T = p.T, L = p.L, NB = p.NI * beam;
+    const int src = p.res_src[res];
+    const int len = src < 0 ? 0 : p.res_len[res];
+    if (threadIdx.x == 0 && len > 0) {
+        int t = len - 1, j;
+        if (p.res_complete[img]) {   // completed at step len - 1 from live row comp_prov
+            const int b = p.comp_prov[(size_t)img * beam + src];
+            rows_s[t] = b;
+            p_s[t] = p.comp_p[(size_t)img * beam + src];
+            j = b;
+            --t;
+        } else {
+            j = src;                 // partial beam src after the last step
+        }
+        for (; t >= 0; --t) {
+            const size_t hi = (size_t)t * NB + (size_t)img * beam + j;
+            const int r = p.hist_parent[hi];
+            rows_s[t] = r;
+            p_s[t] = p.hist_p[hi];
+            j = r;
+        }
+    }
+    __syncthreads();
+    if (p.res_probs)
+        for (int t = threadIdx.x; t < T; t += blockDim.x) p.res_probs[(size_t)res * T + t] = t < len ? p_s[t] : 0.f;
+    if (p.res_alpha) {
+        float* dst = p.res_alpha + (size_t)res * T * L;
+        for (int u = threadIdx.x; u < T * L; u += blockDim.x) {
+            const int t = u / L, l = u - t * L;
+            float v = 0.f;
+            if (t < len) {
+                const int G = t == 0 ? 1 : beam;
+                v = p.hist_alpha[((size_t)t * NB + (size_t)img * G + rows_s[t]) * L + l];
+            }
+            dst[u] = v;
+        }
+    }
 }
 
 cudaError_t beam_update_launch(const BeamParams& p, cudaStream_t st) {
@@ -346,6 +410,12 @@ cudaError_t beam_update_launch(const BeamParams& p, cudaStream_t st) {
 }
 cudaError_t beam_finalize_launch(const BeamParams& p, cudaStream_t st) {
     beam_finalize_kernel<<<(p.NI + 63) / 64, 64, 0, st>>>(p);
+    return cudaGetLastError();
+}
+
+cudaError_t beam_maps_launch(const BeamParams& p, cudaStream_t st) {
+    if (!p.res_src || p.T > 1024) return cudaErrorInvalidValue;
+    beam_maps_kernel<<<p.NI * p.beam, 256, (size_t)p.T * sizeof(int), st>>>(p);
     return cudaGetLastError();
 }
 

@@ -22,6 +22,8 @@ struct RowsParams {
     int topk;             // 0 or beam+1
     int32_t* topk_idx;    // [rows, topk]
     float* topk_p;        // [rows, topk]
+    float* word_probs;    // [rows, tokens_ld] or null: word_probs[row, step] = softmax[next word]
+                          // (0 for a forced word outside [0, V))
 };
 
 struct PItem;
@@ -48,11 +50,22 @@ struct BeamParams {
     double* res_score;        // [NI, beam]
     int32_t* res_n;           // [NI]
     int32_t* res_complete;    // [NI]
+    // per-word maps (null: not requested).  A back-pointer history instead of copies of every beam's maps:
+    const float* hist_alpha;  // [T, NI*beam, L] alpha of step t, rows img*G + g (written by the attention launches)
+    int32_t* hist_parent;     // [T, NI*beam] live row of step t that survivor j of step t came from
+    float* hist_p;            // [T, NI*beam] probability of survivor j's word of step t
+    int32_t* comp_prov;       // [NI, beam] per completed-caption slot: live row it completed from
+    float* comp_p;            // [NI, beam] and the probability of its last word
+    int32_t* res_src;         // [NI, beam] finalize: completed slot / partial beam of result j, -1 if none
+    int L;
+    float* res_alpha;         // [NI, beam, T, L]
+    float* res_probs;         // [NI, beam, T]
 };
 
 cudaError_t rows_softmax_launch(const RowsParams& p, int rows, cudaStream_t st);
 cudaError_t beam_update_launch(const BeamParams& p, cudaStream_t st);
 cudaError_t beam_finalize_launch(const BeamParams& p, cudaStream_t st);
+cudaError_t beam_maps_launch(const BeamParams& p, cudaStream_t st);   // after finalize, when res_alpha / res_probs
 size_t beam_citem_bytes();
 
 }  // namespace sat

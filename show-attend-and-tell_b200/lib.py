@@ -49,6 +49,8 @@ SIGNATURES = {
     "sat_decode_step": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
     "sat_decode_loop": (C.c_int, [_P, _P, _I, _I, _P, _P, _P, _P]),
     "sat_beam_search": (C.c_int, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
+    "sat_decode_loop_maps": (C.c_int, [_P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
+    "sat_beam_search_maps": (C.c_int, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
     "sat_decode_step_host": (C.c_int, [_P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _P]),
     "sat_decode_loop_host": (C.c_int, [_P, _P, _I, _I, _P, _P, _P]),
     "sat_beam_search_host": (C.c_int, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),

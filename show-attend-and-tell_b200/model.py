@@ -65,11 +65,13 @@ def weight_shapes(config):
 
 
 class CaptionData(object):
-    """utils/misc.py:38-60 (memory/output are not returned to the host)."""
-    __slots__ = ("sentence", "score", "complete")
+    """utils/misc.py:38-60 (memory/output are not returned to the host).  With beam_search(with_attention=True):
+    alphas [len, L] (where the model looked for each word) and word_probs [len] (score = their product)."""
+    __slots__ = ("sentence", "score", "complete", "alphas", "word_probs")
 
-    def __init__(self, sentence, score, complete):
+    def __init__(self, sentence, score, complete, alphas=None, word_probs=None):
         self.sentence, self.score, self.complete = sentence, score, complete
+        self.alphas, self.word_probs = alphas, word_probs
 
     def __repr__(self):
         return "CaptionData(score=%.6g, sentence=%s)" % (self.score, self.sentence)
@@ -485,6 +487,25 @@ class CaptionGenerator(object):
         self._keep["loop"] = (contexts, forced_words, tokens, logits)
         return tokens, logits
 
+    def loop_maps_device(self, contexts, num_steps, forced_words=None, want_logits=False, want_alphas=True,
+                         want_word_probs=True):
+        """sat_decode_loop_maps: tokens [B,T], logits [T,B,V] or None, alphas [T,B,L] or None, word_probs [B,T] or None
+        (persistent buffers, overwritten by the next call of the same kind)."""
+        torch = self.torch
+        cfg = self.config
+        B, T = contexts.shape[0], num_steps
+        tokens = self._buf("tokens", (B, T), torch.int32)
+        logits = self._buf("loop_logits", (T, B, cfg.vocabulary_size), torch.float32) if want_logits else None
+        alphas = self._buf("loop_alphas", (T, B, cfg.num_ctx), torch.float32) if want_alphas else None
+        wprobs = self._buf("loop_word_probs", (B, T), torch.float32) if want_word_probs else None
+        self._sync_in()
+        self._check(self.lib.sat_decode_loop_maps(self._h, self._p(contexts), B, T, self._p(forced_words),
+                                                  self._p(tokens), self._p(logits), self._p(alphas), self._p(wprobs),
+                                                  self._st()))
+        self._sync_out()
+        self._keep["loop"] = (contexts, forced_words, tokens, logits, alphas, wprobs)
+        return tokens, logits, alphas, wprobs
+
     def loop_host_submit(self, contexts_host, num_steps, tokens_host, slot, forced_words_host=None):
         """Pipelined host-buffer greedy loop (sat_decode_loop_host_submit): upload on a copy stream, decode,
         download; returns at once.  Pair with loop_host_wait(slot).  Host tensors should be pinned."""
@@ -498,7 +519,9 @@ class CaptionGenerator(object):
         self._check(self.lib.sat_decode_loop_host_wait(self._h, slot))
         return self._keep.pop("pipe%d" % slot)[1]
 
-    def beam_device(self, contexts, beam_size, num_steps, eos_id):
+    def beam_device(self, contexts, beam_size, num_steps, eos_id, with_attention=False):
+        """sat_beam_search (with_attention: sat_beam_search_maps, and alphas [n,beam,T,L], word_probs [n,beam,T]
+        are appended to the returned tuple)."""
         torch = self.torch
         n = contexts.shape[0]
         sent = self._buf("b_sent", (n, beam_size, num_steps), torch.int32)
@@ -507,6 +530,15 @@ class CaptionGenerator(object):
         nres = self._buf("b_nres", (n,), torch.int32)
         comp = self._buf("b_comp", (n,), torch.int32)
         self._sync_in()
+        if with_attention:
+            alphas = self._buf("b_alphas", (n, beam_size, num_steps, self.config.num_ctx), torch.float32)
+            wprobs = self._buf("b_word_probs", (n, beam_size, num_steps), torch.float32)
+            self._check(self.lib.sat_beam_search_maps(self._h, self._p(contexts), n, beam_size, num_steps, eos_id,
+                                                      self._p(sent), self._p(lens), self._p(scores), self._p(nres),
+                                                      self._p(comp), self._p(alphas), self._p(wprobs), self._st()))
+            self._sync_out()
+            self._keep["beam"] = (contexts, sent, lens, scores, nres, comp, alphas, wprobs)
+            return sent, lens, scores, nres, comp, alphas, wprobs
         self._check(self.lib.sat_beam_search(self._h, self._p(contexts), n, beam_size, num_steps, eos_id,
                                              self._p(sent), self._p(lens), self._p(scores), self._p(nres),
                                              self._p(comp), self._st()))
@@ -561,11 +593,33 @@ class CaptionGenerator(object):
             return r
         return r["memory"], r["output"], r["probs"]
 
-    def decode_loop(self, contexts, num_steps=None, forced_words=None, want_logits=False):
+    def decode_loop(self, contexts, num_steps=None, forced_words=None, want_logits=False, want_alphas=False,
+                    want_word_probs=False):
         """initialize + num_steps decode steps without host round trips; returns tokens [B,T]
-        (argmax of every step, model.py:289) and optionally logits [T,B,V]."""
+        (argmax of every step, model.py:289) and optionally logits [T,B,V].
+
+        want_alphas / want_word_probs: return a dict instead, with "tokens", "alphas" [B,T,L] (the attention map of
+        the word emitted at step t) and/or "word_probs" [B,T] (probability of the word fed to step t+1: the argmax, or
+        forced_words[:, t] when teacher forced, which scores a given caption), and "logits" [T,B,V] if want_logits."""
         cfg = self.config
         T = int(num_steps or cfg.max_caption_length)
+        if want_alphas or want_word_probs:
+            is_np = isinstance(contexts, np.ndarray)
+            torch = self.torch
+            ctx = self._dev(contexts, torch.float32)
+            fw = None if forced_words is None else self._dev(forced_words, torch.int32)
+            tokens, logits, alphas, wprobs = self.loop_maps_device(ctx, T, fw, want_logits, want_alphas, want_word_probs)
+            r = dict(tokens=tokens)
+            if want_logits:
+                r["logits"] = logits
+            if want_alphas:
+                r["alphas"] = alphas.transpose(0, 1).contiguous()   # (a copy: the [T,B,L] buffer is reused)
+            if want_word_probs:
+                r["word_probs"] = wprobs
+            if is_np:
+                torch.cuda.synchronize(self.device)
+                return {k: v.cpu().numpy() for k, v in r.items()}
+            return r
         if isinstance(contexts, np.ndarray) and not want_logits:
             B = contexts.shape[0]
             ctx = np.ascontiguousarray(contexts, np.float32)
@@ -585,15 +639,23 @@ class CaptionGenerator(object):
             logits = logits.cpu().numpy() if logits is not None else None
         return (tokens, logits) if want_logits else tokens
 
-    def beam_search(self, contexts, sess=None, vocabulary=None, eos_id=None, beam_size=None, num_steps=None):
+    def beam_search(self, contexts, sess=None, vocabulary=None, eos_id=None, beam_size=None, num_steps=None,
+                    with_attention=False):
         """base_model.py:163-240.  Returns, per image, the captions sorted by descending score
-        (complete captions if any were completed, else the partial ones)."""
+        (complete captions if any were completed, else the partial ones).  with_attention: every CaptionData also
+        carries alphas [len, L] and word_probs [len] (runs on the device whatever the input)."""
         cfg = self.config
         beam = int(beam_size or cfg.beam_size)
         T = int(num_steps or cfg.max_caption_length)
         eos = int(cfg.eos_id if eos_id is None else eos_id)
         n = contexts.shape[0]
-        if isinstance(contexts, np.ndarray):
+        maps = None
+        if with_attention:
+            ts = self.beam_device(self._dev(contexts, self.torch.float32), beam, T, eos, with_attention=True)
+            self.torch.cuda.synchronize(self.device)
+            sent, lens, scores, nres, comp, alphas, wprobs = [t.cpu().numpy() for t in ts]
+            maps = (alphas, wprobs)
+        elif isinstance(contexts, np.ndarray):
             ctx = np.ascontiguousarray(contexts, np.float32)
             sent = np.empty((n, beam, T), np.int32)
             lens = np.empty((n, beam), np.int32)
@@ -609,6 +671,12 @@ class CaptionGenerator(object):
             sent, lens, scores, nres, comp = [t.cpu().numpy() for t in ts]
         results = []
         for k in range(n):
-            results.append([CaptionData([int(w) for w in sent[k, j, :lens[k, j]]], float(scores[k, j]),
-                                        bool(comp[k])) for j in range(int(nres[k]))])
+            caps = []
+            for j in range(int(nres[k])):
+                ln = int(lens[k, j])
+                cd = CaptionData([int(w) for w in sent[k, j, :ln]], float(scores[k, j]), bool(comp[k]))
+                if maps is not None:
+                    cd.alphas, cd.word_probs = maps[0][k, j, :ln].copy(), maps[1][k, j, :ln].copy()
+                caps.append(cd)
+            results.append(caps)
         return results
