@@ -86,7 +86,9 @@ int sat_version(void);
  *                 launch (sat_chain.cu; an experiment, slower than the default chained launches) [0]
  *   "warm"        1 = idle epilogue warps pre-run the epilogue code to warm the instruction caches [1]
  *   "att_wpc"     1 = warp-per-chunk attention kernel for 512-float rows [1]
- *   "att_sms", "att_occ", "att_warps", "l2_w", "l2_vocab", "l2_t", "l2_ctx", "l2_prefetch": grid / cache-policy knobs
+ *   "l2_w"        L2 policy of every dense weight stream: 1 = evict_first, 2 = evict_last, 3 = evict_normal;
+ *                 -1 = evict_first in launches with one row tile (the decode step), evict_last otherwise [-1]
+ *   "att_sms", "att_occ", "att_warps", "l2_vocab", "l2_t", "l2_ctx", "l2_prefetch": grid / cache-policy knobs
  *   "profile"     1 = record CUDA events around every eager kernel launch; read back with sat_get_info
  *                 "prof_ns_<family>" / "prof_n_<family>"
  *   "trace"       1 / 2 / 3 = in-kernel globaltimer stamps of a dense launch ("trace_at") / of the attention kernel /

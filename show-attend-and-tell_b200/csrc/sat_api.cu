@@ -78,7 +78,9 @@ struct sat_handle {
     int dev = 0, num_sms = 0, smem_optin = 0;
     int opt_prologue1 = 1;   // mean of the contexts taken by the packing pass of the projection ("prologue1")
     int opt_gemm = 1, opt_layout = 0, opt_graphs = 1, opt_hoist = 1, opt_coop = 1, opt_xpack = 1;
-    int opt_l2_w = 2, opt_l2_t = 1, opt_l2_ctx = 1;  // weights evict_last; both attention streams evict_first
+    // dense weights: -1 = per launch (see plan()), else one policy for every weight stream; both attention streams
+    // evict_first
+    int opt_l2_w = -1, opt_l2_t = 1, opt_l2_ctx = 1;
     bool weights_locked = false;
 
     Layer init_a1, init_a2, init_b1, init_b2;  // 1-layer mode uses init_a1 / init_b1 as fc_a / fc_b
@@ -623,6 +625,13 @@ static int plan(sat_handle* h, Layer& ly, LinProblem& P, std::initializer_list<L
     P.epi = epi;
     P.out = out;
     P.ldo = ldo;
+    // L2 policy of the weights: evict_first where one CTA row reads each weight tile once per launch (the decode step
+    // at batch <= 128).  A step reads ~137 MB at workload 2 through a 50 MB L2, so no weight survives to the next
+    // step, and weights marked evict_last only displace other data: on an H100 the workload-2 loop runs 8 % faster with
+    // its weights evict_first than evict_last (tools/l2_sweep.py), and an experiment that kept a 16 to 40 MB prefix of
+    // the LSTM / fc_1b / fc_1 / vocabulary weights evict_last was slower than keeping none.  With more than one row
+    // tile, several CTAs read each weight tile in the same launch and L2 serves all but the first: evict_last.
+    P.l2_w = P.n_row_tiles > 1 ? 2 : 1;
     // split-K: fill the SMs; cost model in units of K-blocks (fixed per-CTA overhead ~4)
     const int tiles = P.n_tiles * P.n_row_tiles;
     // split-K: the `splits` CTAs of a tile form one thread-block cluster (partials meet in DSMEM), so the
@@ -683,7 +692,10 @@ static int launch(sat_handle* h, LinProblem* probs, int n, cudaStream_t st) {
     L.layout_mode = h->opt_layout;
     L.stages = lin_pick_stages(max_rt);
     if (h->opt_stages > 0 && h->opt_stages < L.stages) L.stages = h->opt_stages;   // experiment knob: shallower pipeline
-    L.l2_w = (h->cur_tag == kTagDec2 && h->opt_l2_vocab >= 0) ? h->opt_l2_vocab : h->opt_l2_w;   // vocabulary layer: own policy
+    // options "l2_w" / "l2_vocab" (vocabulary layer), when set, replace the policy chosen by plan() / sat_dense_packed
+    const int l2w = (h->cur_tag == kTagDec2 && h->opt_l2_vocab >= 0) ? h->opt_l2_vocab : h->opt_l2_w;
+    if (l2w >= 0)
+        for (int i = 0; i < n; ++i) L.p[i].l2_w = l2w;
     L.dbg = nullptr;
     L.tl = nullptr;
     L.warm_epilogue = h->opt_warm;
@@ -739,6 +751,7 @@ int sat_dense_packed(sat_handle* h, const uint8_t* x_pa, int rows, int row_tile,
     P.splits = splits;
     P.cta_count = P.n_tiles * P.n_row_tiles * splits;
     P.wpack = wpack;
+    P.l2_w = 2;   // (training: every weight stream evict_last)
     P.bias = bias_packed;
     P.epi = epi;
     P.out = out;
@@ -1425,7 +1438,7 @@ static int loop_enqueue_fused(sat_handle* h, const float* ctx, int B, int T, con
         }
         C.layout_mode = h->opt_layout;
         C.stages = stages;
-        C.l2_w = h->opt_l2_w;
+        C.l2_w = h->opt_l2_w >= 0 ? h->opt_l2_w : 2;   // (the chained launch keeps one evict_last policy)
         C.pdl = 1;
         C.row_tile = rtile;
         C.ctr = h->chain_ctr;

@@ -92,7 +92,8 @@ __device__ __forceinline__ void prefetch_l2_bulk(const void* src_gmem, uint32_t 
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src_gmem), "r"(bytes) : "memory");
 }
 // L2 eviction-priority policies for TMA loads: 0 = none, 1 = evict_first (streamed once per step),
-// 2 = evict_last (weights: keep resident in the 50 MB L2 across decode steps), 3 = evict_normal.
+// 2 = evict_last (data re-read while it is still in L2), 3 = evict_normal.  The 50 MB L2 of an H100 cannot keep
+// the weights of a decode step across steps (see plan() in sat_api.cu for the policy of the dense weight streams).
 __device__ __forceinline__ uint64_t l2_policy(int kind) {
     uint64_t pol = 0;
     if (kind == 1) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));

@@ -157,8 +157,8 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_co
     // converged with one elected lane issuing (see elect_one in sat_common.cuh): issued from `if (lane == 0)` code each
     // bulk copy paid register->uniform moves and an indexed walk over the launch descriptor.  Running cursors: no divisions.
     auto stream_half = [&](const bool wside) {
-        const uint64_t wpol = l2_policy(L.l2_w);
-        const int l2w = wside ? L.l2_w : 0;
+        const uint64_t wpol = l2_policy(P.l2_w);
+        const int l2w = wside ? P.l2_w : 0;
         const uint32_t stage0 = smem_u32(stage_base) + (wside ? 0u : (uint32_t)kWStageBytes);
         const uint32_t bar0 = smem_u32(wside ? full_w : full_x);
         const uint32_t bytes = wside ? (uint32_t)kWStageBytes : x_stage_bytes;
@@ -212,12 +212,12 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_co
         if (lane == 0) {
             const uint8_t* src = P.wpack + ((size_t)n_tile * P.k_blocks + kb0) * kWStageBytes;
             const uint8_t* xsrc = P.xpack + ((size_t)rt * P.k_blocks + kb0) * x_stage_bytes;
-            const uint64_t wpol = l2_policy(L.l2_w);
+            const uint64_t wpol = l2_policy(P.l2_w);
             auto load_w = [&](int it) {
                 const int s = it % S;
                 mbar_arrive_expect_tx(&full_w[s], kWStageBytes);
                 tma_bulk_g2s_hint(stage_base + (size_t)s * stage_bytes, src + (size_t)it * kWStageBytes, kWStageBytes,
-                                  &full_w[s], L.l2_w, wpol);
+                                  &full_w[s], P.l2_w, wpol);
             };
             auto load_x = [&](int it) {
                 const int s = it % S;

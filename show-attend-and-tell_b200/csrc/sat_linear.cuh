@@ -54,6 +54,7 @@ struct LinProblem {
     int n_tiles;    // ceil(n_out / 128)
     int splits;     // split-K factor = thread-block cluster size (1, 2, 4 or 8)
     const uint8_t* wpack;  // [n_tiles][k_blocks][hi|lo][128 x 64 bf16, canonical K-major MMA operand layout]
+    int l2_w;              // L2 eviction policy of the weight stream (see l2_policy)
     const float* bias;     // packed output order, n_tiles*128 entries (zero padded); may be null for kEpiNone
     uint8_t* xpack;        // x_mode 1: packed activations [n_row_tiles][k_blocks][hi|lo][row_tile x 64 bf16]
     unsigned* xbar;        // x_mode 1: grid barrier {count, generation}
@@ -96,7 +97,6 @@ struct LinLaunch {
     int nprob;
     int layout_mode;  // 0 = no-swizzle (interleaved 8x16B core matrices), 1 = 128B swizzle
     int stages;
-    int l2_w;         // L2 eviction policy of the weight stream (see l2_policy)
     unsigned long long* dbg;  // optional [grid][16] timeline stamps
     unsigned long long* tl;   // optional {min start, max end} of this launch
     int pdl;          // launched with programmatic stream serialization (see pdl_wait)
