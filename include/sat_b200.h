@@ -161,6 +161,28 @@ int sat_beam_search_maps(sat_handle* h, const float* contexts, int32_t n_img, in
                          int32_t eos_id, int32_t* sentences, int32_t* lengths, double* scores, int32_t* n_results,
                          int32_t* is_complete, float* alphas, float* word_probs, void* stream);
 
+/* Sampling: captions drawn from the model instead of its arg-max (several different captions per image; sampled
+ * captions with the probability of each word for self-critical / REINFORCE fine-tuning and Monte-Carlo scoring).
+ * n_img images x num_samples captions each, drawn word by word from softmax(logits / temperature); the sampled word
+ * is fed to the next step (<start> = 0 first, like sat_decode_loop).  contexts [n_img, L, D] are shared by the
+ * num_samples rows of an image (not replicated).  Row r = image * num_samples + k.
+ * tokens [n_img, num_samples, T] (required); word_probs [n_img, num_samples, T] or NULL: softmax(logits of step t)[w]
+ * at temperature 1 (the model's own probability of the sampled word w, whatever the temperature).  Without word_probs
+ * the vocabulary layer keeps no softmax partials: the draw is all that sampling adds to it.
+ * The draw is the Gumbel-max trick, w = argmax_i(logit_i / temperature - log(-log u(seed, r, t, i))), inside the
+ * fused arg-max of the vocabulary layer (or the per-row kernel when that layer does not fit one wave); u is a
+ * counter-based hash, so the draws are a pure function of (seed, r, t, word): the same call with the same seed gives
+ * the same tokens.  Seed and temperature are not part of the CUDA-graph key: a new seed replays the captured graph.
+ * Errors: SAT_ERR_INVALID for temperature <= 0 or not finite, num_samples < 1, n_img * num_samples > max_batch, T < 1
+ * or a null contexts / tokens (nothing is enqueued); SAT_ERR_UNSUPPORTED for num_samples > 4 (the rows of an image
+ * share its contexts in the attention kernels, which take up to 4; draw more captions with further seeds, as
+ * CaptionGenerator.sample does). */
+int sat_sample_loop(sat_handle* h, const float* contexts, int32_t n_img, int32_t num_samples, int32_t T,
+                    float temperature, uint64_t seed, int32_t* tokens, float* word_probs, void* stream);
+/* the uniform variate behind the Gumbel noise of (seed, row, step, word), u = (bits + 0.5) * 2^-32 in (0, 1), computed
+ * on the host (tests rebuild every draw with it) */
+double sat_sample_uniform(uint64_t seed, int64_t row, int32_t step, int32_t word);
+
 /* host-buffer forms: copy in, run, copy out, synchronise (what a sess.run caller sees) */
 int sat_decode_step_host(sat_handle* h, const float* contexts_host, int32_t contexts_changed,
                          const int32_t* last_word_host, const float* last_memory_host,

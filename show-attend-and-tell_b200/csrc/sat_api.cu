@@ -2,6 +2,7 @@
 // ingestion (TF variable names/layouts, base_model.py:242-278), workspace, and the
 // kernel sequences of prepare / decode step / decode loop / beam search.
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
@@ -57,6 +58,8 @@ struct Layer {
     float* am_sum = nullptr;     // word probabilities: per-tile softmax partials (like am_key), forced-word logits
     float* am_wlogit = nullptr;
     size_t am_sum_n = 0;
+    float2* am_smp = nullptr;    // sampling: per-tile {raw maximum, raw logit of the sampled candidate} (like am_key)
+    size_t am_smp_n = 0;
 };
 
 struct VecParam {  // a kernel of shape [n,1] kept as a plain fp32 vector
@@ -159,6 +162,7 @@ struct sat_handle {
     int chain_clusters[9] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};   // resident clusters of the chained kernel per cluster size
     const unsigned* att_qflag = nullptr;   // set around the attention launch that runs beside a chained launch
     unsigned att_qtarget = 0;
+    SampleParams* smp = nullptr;           // sampling loop: {seed, 1 / temperature}, written before each call (not in graphs)
     void* train = nullptr;                 // training state (sat_train.cu)
     void (*train_free)(void*) = nullptr;
     unsigned long long* trace = nullptr;   // [1024][16] timeline stamps of the last traced launch
@@ -203,6 +207,14 @@ static int dmalloc(T** p, size_t n) {
     return SAT_OK;
 }
 
+// Scratch buffers grow (free + larger allocation) when a call needs more than any call before it.  Every captured graph
+// may hold the old address, so the graphs go with it and are captured again on their next use.
+static void drop_graphs(sat_handle* h) {
+    for (auto& g : h->graphs)
+        if (g.exec) cudaGraphExecDestroy(g.exec);
+    h->graphs.clear();
+}
+
 static int layer_setup(sat_handle* h, Layer& ly, const char* name, int K, int n_out, bool lstm, bool has_bias) {
     ly.name = name;
     ly.K = K;
@@ -229,6 +241,7 @@ static void layer_free(Layer& ly) {
     cudaFree(ly.am_ctr);
     cudaFree(ly.am_sum);
     cudaFree(ly.am_wlogit);
+    cudaFree(ly.am_smp);
     ly = Layer();
 }
 
@@ -275,7 +288,7 @@ extern "C" void sat_destroy(sat_handle* h) {
                     h->rowcnt, h->topk_idx, h->part_n, h->comp_n, h->comp_sent, h->sent[0], h->sent[1], h->topk_p,
                     h->part_score, h->comp_heap, h->stage_ctx, h->stage_misc, h->att_part, h->trace, h->pa_h[0], h->pa_h[1], h->pa_z, h->pa_emb, h->pa_t, h->pa_z2[1], h->z2[1],
                     h->chain_ctr, h->chain_scratch, h->chain_best, h->hist_alpha, h->hist_p, h->comp_p, h->hist_parent,
-                    h->comp_prov, h->res_src};
+                    h->comp_prov, h->res_src, h->smp};
     for (void* b : bufs) cudaFree(b);
     delete h;
 }
@@ -657,6 +670,7 @@ static int plan(sat_handle* h, Layer& ly, LinProblem& P, std::initializer_list<L
     if (xneed > ly.xpack_bytes || !ly.xbar) {
         if (stream_capturing(st)) return fail(SAT_ERR_STATE, "%s: scratch growth during graph capture", ly.name.c_str());
         CK(cudaDeviceSynchronize());
+        drop_graphs(h);   // captured graphs hold the buffer freed below
         cudaFree(ly.xpack);
         ly.xpack = nullptr;
         ly.xpack_bytes = 0;
@@ -937,6 +951,7 @@ static int attention_impl(sat_handle* h, const float* ctx, int n_img, int G, con
     if (pneed > h->att_part_floats) {
         if (stream_capturing(st)) return fail(SAT_ERR_STATE, "attention scratch growth during graph capture");
         CK(cudaDeviceSynchronize());
+        drop_graphs(h);   // captured graphs hold the buffer freed below
         cudaFree(h->att_part);
         h->att_part = nullptr;
         h->att_part_floats = 0;
@@ -1005,6 +1020,7 @@ static int attach_argmax(sat_handle* h, Layer& ly, LinProblem& P, const RowsPara
     if (need > ly.am_n) {
         if (stream_capturing(st)) return fail(SAT_ERR_STATE, "%s: scratch growth during graph capture", ly.name.c_str());
         CK(cudaDeviceSynchronize());
+        drop_graphs(h);   // captured graphs hold the buffer freed below
         cudaFree(ly.am_key);
         ly.am_key = nullptr; ly.am_n = 0;
         RET(dmalloc(&ly.am_key, need));
@@ -1017,6 +1033,7 @@ static int attach_argmax(sat_handle* h, Layer& ly, LinProblem& P, const RowsPara
     if (am->word_probs && ly.am_sum_n < ly.am_n) {   // (only handles that ask for word probabilities)
         if (stream_capturing(st)) return fail(SAT_ERR_STATE, "%s: scratch growth during graph capture", ly.name.c_str());
         CK(cudaDeviceSynchronize());
+        drop_graphs(h);   // captured graphs hold the buffer freed below
         cudaFree(ly.am_sum);
         cudaFree(ly.am_wlogit);
         ly.am_sum = ly.am_wlogit = nullptr; ly.am_sum_n = 0;
@@ -1024,12 +1041,25 @@ static int attach_argmax(sat_handle* h, Layer& ly, LinProblem& P, const RowsPara
         RET(dmalloc(&ly.am_wlogit, (size_t)h->max_rows));
         ly.am_sum_n = ly.am_n;
     }
+    if (am->sample && am->word_probs && ly.am_smp_n < ly.am_n) {   // (only handles that sample with word probabilities)
+        if (stream_capturing(st)) return fail(SAT_ERR_STATE, "%s: scratch growth during graph capture", ly.name.c_str());
+        CK(cudaDeviceSynchronize());
+        drop_graphs(h);   // captured graphs hold the buffer freed below
+        cudaFree(ly.am_smp);
+        ly.am_smp = nullptr; ly.am_smp_n = 0;
+        RET(dmalloc(&ly.am_smp, ly.am_n));
+        ly.am_smp_n = ly.am_n;
+    }
     P.am_key = ly.am_key; P.am_ctr = ly.am_ctr;
     P.am_tokens = am->tokens; P.am_tokens_ld = am->tokens_ld; P.am_step = am->step;
     P.am_next_word = am->next_word; P.am_forced = am->forced; P.am_forced_ld = am->forced_ld;
     if (am->word_probs) {
         P.am_probs = am->word_probs; P.am_probs_ld = am->tokens_ld;
         P.am_sum = ly.am_sum; P.am_wlogit = ly.am_wlogit;
+    }
+    if (am->sample) {   // without word probabilities the sampling instance keeps no softmax partials
+        P.smp = am->sample;
+        if (am->word_probs) P.am_smp = ly.am_smp;
     }
     return 1;
 }
@@ -1217,15 +1247,35 @@ static int run_graphed(sat_handle* h, const std::vector<long long>& key, cudaStr
 // alphas [T,B,L] / word_probs [B,T] (may be null): the per-word maps of sat_decode_loop_maps
 static float* step_alpha(float* alphas, int t, int B, int L) { return alphas ? alphas + (size_t)t * B * L : nullptr; }
 
+// Prologue of a loop over B = n_img x G rows: project the contexts and run initialize once per image; with G > 1
+// (several sampled captions per image) every row then gets its image's initial state, and the packed h0 is built for the
+// row tile of B rows.
+static int loop_prologue(sat_handle* h, const float* ctx, int B, int G, cudaStream_t st, uint8_t* h0_pa) {
+    if (G == 1) return prepare_impl(h, ctx, B, h->st_c[0], h->st_h[0], st, h0_pa);
+    const int H = h->d.num_lstm_units;
+    RET(prepare_impl(h, ctx, B / G, h->st_c[1], h->st_h[1], st));   // (slot 1 is free until step 0 writes it)
+    CK(bcast_state_launch(h->st_c[1], h->st_h[1], h->st_c[0], h->st_h[0], B, G, H, st));
+    h->launches += 1;
+    if (h0_pa) {
+        PackJob job{h->st_h[0], nullptr, H, H, B, row_tile_for(B), h0_pa};
+        CK(pack_rows_launch(&job, 1, h->opt_layout, st));
+        h->launches += 1;
+    }
+    return SAT_OK;
+}
+
+// G: rows per image (sampling: captions per image; the attention kernels share an image's contexts between them);
+// smp: the sampling loop's {seed, 1 / temperature} (null: greedy / teacher forced)
 static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, const int32_t* forced, int32_t* tokens,
-                                float* logits_all, float* alphas, float* word_probs, cudaStream_t st) {
+                                float* logits_all, float* alphas, float* word_probs, cudaStream_t st, int G = 1,
+                                const SampleParams* smp = nullptr) {
     if (!h->side) {
         CK(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
     }
     const sat_dims& d = h->d;
-    RET(prepare_impl(h, ctx, B, h->st_c[0], h->st_h[0], st, h->pa_h[0]));
+    RET(loop_prologue(h, ctx, B, G, st, h->pa_h[0]));
     CK(cudaMemsetAsync(h->word, 0, (size_t)B * sizeof(int32_t), st));  // <start> = 0 (model.py:254)
     for (int t = 0; t < T; ++t) {
         const float *c_in = h->st_c[t & 1], *h_in = h->st_h[t & 1];
@@ -1236,7 +1286,7 @@ static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, c
         float* zcur = h->z2[t & 1];          // context vector of this step (fp32 + packed), written by attention(t)
         h->pa_cur_z = h->pa_z2[t & 1];
         if (t == 0)   // q(0), attention(0) and the embedding of <start>
-            RET(attention_impl(h, ctx, B, 1, h_in, step_alpha(alphas, 0, B, d.num_ctx), zcur, st, false, h->word));
+            RET(attention_impl(h, ctx, B / G, G, h_in, step_alpha(alphas, 0, B, d.num_ctx), zcur, st, false, h->word));
         RET(lstm_impl(h, zcur, h->word, c_in, h_in, c_out, h_out, B, st));
         float* logits = logits_all ? logits_all + (size_t)t * B * d.vocabulary_size : h->logits;
         if (t + 1 < T) {
@@ -1254,7 +1304,7 @@ static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, c
             // the SMs left over
             int budget = h->opt_att_sms > 0 ? h->opt_att_sms : h->num_sms - h->dec_2.n_tiles;
             if (budget < h->num_sms / 4) budget = h->num_sms;
-            RET(attention_impl(h, ctx, B, 1, h_out, step_alpha(alphas, t + 1, B, d.num_ctx), h->z2[(t + 1) & 1], h->side,
+            RET(attention_impl(h, ctx, B / G, G, h_out, step_alpha(alphas, t + 1, B, d.num_ctx), h->z2[(t + 1) & 1], h->side,
                                true, nullptr, budget));
             CK(cudaEventRecord(h->ev_join, h->side));
             h->pa_cur_h_in = h->pa_h[t & 1];
@@ -1265,6 +1315,7 @@ static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, c
         memset(&rp, 0, sizeof(rp));
         rp.tokens = tokens; rp.tokens_ld = T; rp.step = t;
         rp.next_word = h->word; rp.forced = forced; rp.forced_ld = T; rp.word_probs = word_probs;
+        rp.sample = smp;
         int fused = 0;
         RET(decode_impl(h, h_out, zcur, h->word, logits, B, st, false, &rp, &fused, 2, t + 1 < T));  // fc_2 + argmax
         if (!fused) {
@@ -1285,9 +1336,10 @@ static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, c
 // grid leaves idle and the two run side by side without a second stream; it only waits for its predecessor
 // right before it exits, which keeps "kernel k complete => kernel k-1 complete" for the LSTM that follows.
 static int loop_enqueue_chain(sat_handle* h, const float* ctx, int B, int T, const int32_t* forced, int32_t* tokens,
-                              float* logits_all, float* alphas, float* word_probs, cudaStream_t st, bool prepared = false) {
+                              float* logits_all, float* alphas, float* word_probs, cudaStream_t st, bool prepared = false,
+                              int G = 1, const SampleParams* smp = nullptr) {
     const sat_dims& d = h->d;
-    if (!prepared) RET(prepare_impl(h, ctx, B, h->st_c[0], h->st_h[0], st, h->pa_h[0]));
+    if (!prepared) RET(loop_prologue(h, ctx, B, G, st, h->pa_h[0]));
     CK(cudaMemsetAsync(h->word, 0, (size_t)B * sizeof(int32_t), st));  // <start> = 0 (model.py:254)
     int budget = h->opt_att_sms > 0 ? h->opt_att_sms : h->num_sms - h->dec_2.n_tiles;
     if (budget < h->num_sms / 4) budget = h->num_sms;
@@ -1299,7 +1351,7 @@ static int loop_enqueue_chain(sat_handle* h, const float* ctx, int B, int T, con
         h->pa_cur_h_out = h->pa_h[(t + 1) & 1];
         h->pa_cur_z = h->pa_z;
         if (t == 0)   // q(0), attention(0) and the embedding of <start>
-            RET(attention_impl(h, ctx, B, 1, h_in, step_alpha(alphas, 0, B, d.num_ctx), h->z, st, false, h->word));
+            RET(attention_impl(h, ctx, B / G, G, h_in, step_alpha(alphas, 0, B, d.num_ctx), h->z, st, false, h->word));
         RET(lstm_impl(h, h->z, h->word, c_in, h_in, c_out, h_out, B, st));
         float* logits = logits_all ? logits_all + (size_t)t * B * d.vocabulary_size : h->logits;
         RET(decode_impl(h, h_out, h->z, h->word, logits, B, st, t + 1 < T, nullptr, nullptr, 1));   // fc_1 || q(t+1)
@@ -1307,6 +1359,7 @@ static int loop_enqueue_chain(sat_handle* h, const float* ctx, int B, int T, con
         memset(&rp, 0, sizeof(rp));
         rp.tokens = tokens; rp.tokens_ld = T; rp.step = t;
         rp.next_word = h->word; rp.forced = forced; rp.forced_ld = T; rp.word_probs = word_probs;
+        rp.sample = smp;
         int fused = 0;
         RET(decode_impl(h, h_out, h->z, h->word, logits, B, st, false, &rp, &fused, 2, t + 1 < T));  // fc_2 + argmax
         if (!fused) {
@@ -1315,7 +1368,7 @@ static int loop_enqueue_chain(sat_handle* h, const float* ctx, int B, int T, con
         }
         if (t + 1 < T) {
             h->pa_cur_h_in = h->pa_h[(t + 1) & 1];
-            RET(attention_impl(h, ctx, B, 1, h_out, step_alpha(alphas, t + 1, B, d.num_ctx), h->z, st, true, nullptr, budget,
+            RET(attention_impl(h, ctx, B / G, G, h_out, step_alpha(alphas, t + 1, B, d.num_ctx), h->z, st, true, nullptr, budget,
                                true));
         }
     }
@@ -1496,23 +1549,25 @@ static bool vocab_argmax_fits(sat_handle* h, int B) {
     return h->dec_2.n_tiles * ((B + kMaxRowTile - 1) / kMaxRowTile) <= h->num_sms;
 }
 
+// G, smp: see loop_enqueue_overlap (the sampling loop runs G = num_samples rows per image)
 static int loop_enqueue(sat_handle* h, const float* ctx, int B, int T, const int32_t* forced, int32_t* tokens,
-                        float* logits_all, float* alphas, float* word_probs, cudaStream_t st) {
+                        float* logits_all, float* alphas, float* word_probs, cudaStream_t st, int G = 1,
+                        const SampleParams* smp = nullptr) {
     const bool pa = h->pa_ok && h->opt_pa && h->opt_gemm != 0;
     const bool am = pa && vocab_argmax_fits(h, B);
-    const bool maps = alphas || word_probs;   // (the experimental chained launch takes no maps)
-    if (!maps && fused_loop_available(h, B)) return loop_enqueue_fused(h, ctx, B, T, forced, tokens, logits_all, st, false);
+    const bool maps = alphas || word_probs;   // (the experimental chained launch takes no maps, and does not sample)
+    if (!maps && !smp && fused_loop_available(h, B)) return loop_enqueue_fused(h, ctx, B, T, forced, tokens, logits_all, st, false);
     if (am && h->opt_overlap == 2 && h->opt_pdl && h->d.num_decode_layers == 2)
-        return loop_enqueue_chain(h, ctx, B, T, forced, tokens, logits_all, alphas, word_probs, st);
+        return loop_enqueue_chain(h, ctx, B, T, forced, tokens, logits_all, alphas, word_probs, st, false, G, smp);
     if (am && h->opt_overlap && h->d.num_decode_layers == 2 && st != nullptr && st != cudaStreamLegacy)
-        return loop_enqueue_overlap(h, ctx, B, T, forced, tokens, logits_all, alphas, word_probs, st);
-    RET(prepare_impl(h, ctx, B, h->st_c[0], h->st_h[0], st, pa ? h->pa_h[0] : nullptr));
+        return loop_enqueue_overlap(h, ctx, B, T, forced, tokens, logits_all, alphas, word_probs, st, G, smp);
+    RET(loop_prologue(h, ctx, B, G, st, pa ? h->pa_h[0] : nullptr));
     CK(cudaMemsetAsync(h->word, 0, (size_t)B * sizeof(int32_t), st));  // <start> = 0 (model.py:254)
     bool emb_valid = false;
     for (int t = 0; t < T; ++t) {
         StepIO io;
         memset(&io, 0, sizeof(io));
-        io.ctx = ctx; io.n_img = B; io.group = 1; io.last_word = h->word;
+        io.ctx = ctx; io.n_img = B / G; io.group = G; io.last_word = h->word;
         io.c_in = h->st_c[t & 1]; io.h_in = h->st_h[t & 1];
         io.c_out = h->st_c[(t + 1) & 1]; io.h_out = h->st_h[(t + 1) & 1];
         io.logits = logits_all ? logits_all + (size_t)t * B * h->d.vocabulary_size : nullptr;
@@ -1521,6 +1576,7 @@ static int loop_enqueue(sat_handle* h, const float* ctx, int B, int T, const int
         io.rows.tokens = tokens; io.rows.tokens_ld = T; io.rows.step = t;
         io.rows.next_word = h->word; io.rows.forced = forced; io.rows.forced_ld = T;
         io.rows.word_probs = word_probs;
+        io.rows.sample = smp;
         io.q_ready = t > 0;
         io.make_next_q = t + 1 < T;
         io.pa_slot = t & 1;          // initialize / the previous LSTM wrote the packed h into this slot
@@ -1624,6 +1680,43 @@ extern "C" int sat_decode_loop_maps(sat_handle* h, const float* contexts, int32_
     // record of what T1 holds must follow in every case (eager, capture, replay), or a later single step on other
     // contexts would skip its projection.
     note_projected(h, rc == SAT_OK ? contexts : nullptr, B);
+    return rc;
+}
+
+// ------------------------------------------------------------ sampling
+extern "C" double sat_sample_uniform(uint64_t seed, int64_t row, int32_t step, int32_t word) {
+    const uint32_t bits = sample_bits(sample_key(seed, row, step), word);
+    return ((double)bits + 0.5) * 2.3283064365386963e-10;   // (bits + 1/2) 2^-32: exact in fp64
+}
+
+extern "C" int sat_sample_loop(sat_handle* h, const float* contexts, int32_t n_img, int32_t num_samples, int32_t T,
+                               float temperature, uint64_t seed, int32_t* tokens, float* word_probs, void* stream) {
+    if (!h) return fail(SAT_ERR_INVALID, "null handle");
+    if (!contexts || !tokens) return fail(SAT_ERR_INVALID, "sat_sample_loop: null tensor");
+    if (!(temperature > 0.0f) || !isfinite(temperature) || !isfinite(1.0f / temperature))
+        return fail(SAT_ERR_INVALID, "temperature %g must be positive and finite", (double)temperature);
+    if (num_samples < 1) return fail(SAT_ERR_INVALID, "num_samples %d < 1", num_samples);
+    if (n_img < 1 || (long long)n_img * num_samples > h->max_rows)
+        return fail(SAT_ERR_INVALID, "n_img*num_samples %lld outside [1, %d]", (long long)n_img * num_samples, h->max_rows);
+    if (T < 1) return fail(SAT_ERR_INVALID, "T must be >= 1");
+    // the rows of an image share its contexts inside the attention kernels, which take up to 4 rows per image
+    if (num_samples > 4) return fail(SAT_ERR_UNSUPPORTED, "num_samples %d > 4 (draw more with further seeds)", num_samples);
+    RET(require_ready(h));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!h->smp) {
+        if (stream_capturing(st)) return fail(SAT_ERR_STATE, "sat_sample_loop: allocation during graph capture");
+        RET(dmalloc(&h->smp, 1));
+    }
+    // seed and temperature live in device memory, written here outside any capture: a graph captured for these buffers
+    // replays with any seed or temperature
+    CK(sample_params_launch(h->smp, seed, 1.0f / temperature, st));
+    h->launches += 1;
+    const int B = n_img * num_samples;
+    std::vector<long long> key = {5, (long long)contexts, n_img, num_samples, T, (long long)tokens, (long long)word_probs};
+    const int rc = run_graphed(h, key, st, [&]() -> int {
+        return loop_enqueue(h, contexts, B, T, nullptr, tokens, nullptr, nullptr, word_probs, st, num_samples, h->smp);
+    });
+    note_projected(h, rc == SAT_OK ? contexts : nullptr, n_img);   // (see sat_decode_loop)
     return rc;
 }
 

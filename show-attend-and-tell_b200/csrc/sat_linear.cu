@@ -88,8 +88,11 @@ struct XChunk {
 // NT = (row tile of the launch) / 16: the accumulator fragments per warpgroup
 // WP: the fused arg-max also produces the probability of the word fed to the next step (LinProblem::am_probs); a
 // separate instance, so that launches without it run the code they ran before
-template <int NT, bool WP>
+// SMP: sampling — the arg-max ranks logit / temperature + Gumbel noise (LinProblem::smp); instances of their own,
+// with WP (the sampled word's probability) or without it (no softmax partials: nothing but the draw is added)
+template <int NT, bool WP, bool SMP = false>
 __global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_constant__ LinLaunch L) {
+    constexpr bool SWP = SMP && WP;   // sampling with word probabilities: the raw logits ride beside the keys
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // control block: barriers etc. live in the first 1024 bytes
     uint64_t* full_w = reinterpret_cast<uint64_t*>(smem_raw);  // [stages]
@@ -565,6 +568,30 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_co
                     // running 64-bit max: two independent chains of 2-instruction steps instead of one chain of
                     // compare / compare / select per element
                     unsigned long long k0 = 0ull, k1 = 0ull;
+                    float mr = -INFINITY;   // (SWP) raw maximum: the keys rank the perturbed values
+                    if constexpr (SMP) {
+                        // the draw of (seed, row, step, word): key once per row, one hash + two logarithms per logit
+                        const SampleKey sk = sample_key(P.smp->seed, row0 + r, P.am_step);
+                        const float itau = P.smp->inv_tau;
+                        auto draw = [&](float v, int i) -> unsigned long long {
+                            return i < n_out ? argmax_key(fmaf(v, itau, sample_gumbel(sample_bits(sk, i))), i) : 0ull;
+                        };
+                        // (the warm-up pass runs before the main loop of its warps: one unrolled iteration warms the
+                        // code, all eight would hold the MMAs back by the cost of the draw)
+                        const int jn = dry ? 2 : 8;
+#pragma unroll 2
+                        for (int j = 0; j < jn; ++j) {
+                            const int jj = (j + pt) & 7;
+                            const float4 a4 = row_t[jj];
+                            const int i0 = n_tile * kTileN + part * 32 + jj * 4;
+                            k0 = max(k0, max(draw(a4.x, i0 + 0), draw(a4.y, i0 + 1)));
+                            k1 = max(k1, max(draw(a4.z, i0 + 2), draw(a4.w, i0 + 3)));
+                            if constexpr (WP) {
+                                mr = fmaxf(mr, fmaxf(i0 + 0 < n_out ? a4.x : -INFINITY, i0 + 1 < n_out ? a4.y : -INFINITY));
+                                mr = fmaxf(mr, fmaxf(i0 + 2 < n_out ? a4.z : -INFINITY, i0 + 3 < n_out ? a4.w : -INFINITY));
+                            }
+                        }
+                    } else {
 #pragma unroll 2
                     for (int j = 0; j < 8; ++j) {
                         const int jj = (j + pt) & 7;
@@ -577,13 +604,21 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_co
                         k0 = max(k0, max(e0, e1));
                         k1 = max(k1, max(e2, e3));
                     }
+                    }
                     unsigned long long key = max(k0, k1);
                     key = max(key, __shfl_xor_sync(0xffffffffu, key, 1));
                     key = max(key, __shfl_xor_sync(0xffffffffu, key, 2));
                     if (live && part == 0 && !dry) am_key[r] = key;
                     if constexpr (WP) {
-                        // softmax partial of the row over this tile, relative to the tile maximum (the key's value)
-                        const float mt = argmax_key_value(key);
+                        // softmax partial of the row over this tile, relative to the tile maximum (the key's value;
+                        // sampling: the raw maximum)
+                        float mt;
+                        if constexpr (SMP) {
+                            mt = fmaxf(mr, __shfl_xor_sync(0xffffffffu, mr, 1));
+                            mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+                        } else {
+                            mt = argmax_key_value(key);
+                        }
                         float s = 0.f;
 #pragma unroll 2
                         for (int j = 0; j < 8; ++j) {
@@ -600,7 +635,11 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_co
                         if (live && part == 0) {
                             float* const am_sum = P.am_sum + (size_t)(rt * P.n_tiles + n_tile) * N;
                             if (!dry) am_sum[r] = s;
-                            if (P.am_forced) {   // teacher forcing: the tile that owns the forced word keeps its logit
+                            if constexpr (SMP) {   // the tile's sampled candidate keeps its raw logit beside the key
+                                const int c = (argmax_key_index(key) - n_tile * kTileN) & (kTileN - 1);
+                                const float lw = row_base[r * row_mul + c];
+                                if (!dry) P.am_smp[(size_t)(rt * P.n_tiles + n_tile) * N + r] = make_float2(mt, lw);
+                            } else if (P.am_forced) {   // teacher forcing: the tile that owns the forced word keeps its logit
                                 const int w = P.am_forced[(size_t)(row0 + r) * P.am_forced_ld + P.am_step];
                                 const int c = w - n_tile * kTileN;
                                 if (c >= 0 && c < kTileN && w < n_out) {
@@ -649,31 +688,53 @@ __global__ void __launch_bounds__(kLinThreads, 1) lin_mma_kernel(const __grid_co
                     const unsigned long long* pk = P.am_key + (size_t)rt2 * n_tiles * N + cc;
                     unsigned long long best = 0ull;
                     float lm = -INFINITY, ls = 0.f;   // (WP) merged softmax partials of this thread's tiles
+                    float braw = 0.f;                 // (SWP) raw logit of the best candidate
                     for (int tl = pt; tl < n_tiles; tl += kLinProducers) {
                         const unsigned long long k = __ldcg(pk + (size_t)tl * N);
+                        if constexpr (SWP) {
+                            const float2 ms = __ldcg(P.am_smp + (pk - P.am_key) + (size_t)tl * N);
+                            if (k > best) braw = ms.y;
+                            best = max(best, k);
+                            lse_merge(lm, ls, ms.x, __ldcg(P.am_sum + (pk - P.am_key) + (size_t)tl * N));
+                        } else {
                         best = max(best, k);
                         if constexpr (WP) lse_merge(lm, ls, argmax_key_value(k), __ldcg(P.am_sum + (pk - P.am_key) + (size_t)tl * N));
+                        }
                     }
 #pragma unroll
                     for (int o = 16; o > 0; o >>= 1) {
+                        if constexpr (SWP) {
+                            const unsigned long long ob = __shfl_xor_sync(0xffffffffu, best, o);
+                            const float orw = __shfl_xor_sync(0xffffffffu, braw, o);
+                            if (ob > best) { best = ob; braw = orw; }
+                        } else {
                         best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
+                        }
                         if constexpr (WP) lse_merge(lm, ls, __shfl_xor_sync(0xffffffffu, lm, o), __shfl_xor_sync(0xffffffffu, ls, o));
                     }
                     float2* const red_ms = reinterpret_cast<float2*>(smem_raw + 384);   // [8] (between red_s and the scratch line)
+                    float* const red_raw = reinterpret_cast<float*>(smem_raw + 448);    // [8] (SWP)
                     if ((pt & 31) == 0) {
                         red_s[pt >> 5] = best;
                         if constexpr (WP) red_ms[pt >> 5] = make_float2(lm, ls);
+                        if constexpr (SWP) red_raw[pt >> 5] = braw;
                     }
                     named_bar_sync(1, kLinProducers);
                     if (pt == 0) {
 #pragma unroll
                         for (int w = 1; w < kLinProducers / 32; ++w) {
+                            if constexpr (SWP) {
+                                if (red_s[w] > best) braw = red_raw[w];
+                            }
                             best = max(best, red_s[w]);
                             if constexpr (WP) lse_merge(lm, ls, red_ms[w].x, red_ms[w].y);
                         }
                         const int bi2 = argmax_key_index(best);
                         const int nw = P.am_forced ? P.am_forced[(size_t)r * P.am_forced_ld + P.am_step] : bi2;
-                        if constexpr (WP) {
+                        if constexpr (SWP) {
+                            // softmax(logits)[w] at temperature 1 of the sampled word w: lm is the raw row maximum
+                            if (!dry) P.am_probs[(size_t)r * P.am_probs_ld + P.am_step] = expf(braw - lm) / ls;
+                        } else if constexpr (WP) {
                             // softmax(logits)[nw] = exp(l_nw - M) / S; M is the row maximum (lm == its value); a forced
                             // word outside [0, V) has probability 0 and is never used as an index
                             float pw = 0.f;
@@ -933,11 +994,18 @@ int device_sm_count() {
 
 static int g_smem_optin = 0;
 
-static void (*const g_lin_kernels[2][kMaxRowTile / 16])(LinLaunch) = {
+// [plain, word probabilities, sampling with word probabilities, sampling][row tile / 16 - 1]
+static void (*const g_lin_kernels[4][kMaxRowTile / 16])(LinLaunch) = {
     {lin_mma_kernel<1, false>, lin_mma_kernel<2, false>, lin_mma_kernel<3, false>, lin_mma_kernel<4, false>,
      lin_mma_kernel<5, false>, lin_mma_kernel<6, false>, lin_mma_kernel<7, false>, lin_mma_kernel<8, false>},
     {lin_mma_kernel<1, true>, lin_mma_kernel<2, true>, lin_mma_kernel<3, true>, lin_mma_kernel<4, true>,
-     lin_mma_kernel<5, true>, lin_mma_kernel<6, true>, lin_mma_kernel<7, true>, lin_mma_kernel<8, true>}};
+     lin_mma_kernel<5, true>, lin_mma_kernel<6, true>, lin_mma_kernel<7, true>, lin_mma_kernel<8, true>},
+    {lin_mma_kernel<1, true, true>, lin_mma_kernel<2, true, true>, lin_mma_kernel<3, true, true>,
+     lin_mma_kernel<4, true, true>, lin_mma_kernel<5, true, true>, lin_mma_kernel<6, true, true>,
+     lin_mma_kernel<7, true, true>, lin_mma_kernel<8, true, true>},
+    {lin_mma_kernel<1, false, true>, lin_mma_kernel<2, false, true>, lin_mma_kernel<3, false, true>,
+     lin_mma_kernel<4, false, true>, lin_mma_kernel<5, false, true>, lin_mma_kernel<6, false, true>,
+     lin_mma_kernel<7, false, true>, lin_mma_kernel<8, false, true>}};
 
 cudaError_t lin_init_attrs() {
     int dev = 0;
@@ -984,6 +1052,11 @@ cudaError_t lin_launch(const LinLaunch& L, cudaStream_t st, bool use_simt) {
             if (!L.p[i].am_key || !L.p[i].am_sum || L.p[i].splits != 1 || (L.p[i].am_forced && !L.p[i].am_wlogit))
                 return cudaErrorInvalidValue;
             wp = 1;
+        }
+        if (L.p[i].smp) {
+            if (!L.p[i].am_key || L.p[i].splits != 1 || L.p[i].am_forced || (L.p[i].am_probs && !L.p[i].am_smp))
+                return cudaErrorInvalidValue;
+            wp = L.p[i].am_probs ? 2 : 3;
         }
         if (L.p[i].row_tile > max_rt) max_rt = L.p[i].row_tile;
         // (one MMA width per launch: grouped problems share the row tile, so no MMA reads past its operand)

@@ -42,6 +42,8 @@ struct LinSeg {
 // consuming dense layer fetches its X stages by TMA with no conversion pass.
 __host__ __device__ __forceinline__ size_t pa_stage_bytes(int row_tile) { return (size_t)row_tile * kBK * 2 * 2; }
 
+struct SampleParams;   // sampling loop: see sample_key below
+
 struct LinProblem {
     LinSeg seg[kMaxSeg];
     int nseg;
@@ -90,6 +92,11 @@ struct LinProblem {
     uint8_t* am_emb_pa;    // packed [rows, E]
     int cta_begin;         // first CTA of this problem in the grouped grid
     int cta_count;
+    // optional sampling (sat_sample_loop): the fused arg-max picks argmax_i(logit_i / temperature + g(seed, row, step, i))
+    // (Gumbel-max: a draw from softmax(logits / temperature)); the softmax partials stay on the raw logits.  Runs a
+    // sampling instance of the kernel (lin_launch picks it when smp is set); with am_probs also am_sum and am_smp.
+    const SampleParams* smp;   // device {seed, 1 / temperature}: read at run time, so graphs replay any seed
+    float2* am_smp;        // laid out like am_key: {raw tile maximum, raw logit of the tile's sampled candidate}
 };
 
 struct LinLaunch {
@@ -218,6 +225,54 @@ __host__ __device__ inline DropGen drop_gen(unsigned long long seed, unsigned lo
     g.kt = kt;
     return g;
 }
+// Counter-based generator of the sampling loop (sat_sample_loop): the uniform variate of (seed, row, step, word) is
+// u = (bits + 0.5) * 2^-32, strictly inside (0, 1), with bits a 32-bit hash; g = -log(-log u) is its Gumbel(0, 1) noise.
+// (seed, row, step) is mixed once per row by two rounds of splitmix64 into a 64-bit key; each word then costs one
+// keyed 32-bit hash (lowbias32 with the key's halves entering before the first and between the two multiplies, a
+// bijection of the word for a given key).  sat_sample_uniform is this function on the host.
+struct SampleParams {
+    unsigned long long seed;
+    float inv_tau;          // 1 / temperature
+    float pad;
+};
+struct SampleKey {
+    uint32_t k0, k1;
+};
+__host__ __device__ inline unsigned long long splitmix64(unsigned long long z) {
+    z += 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+__host__ __device__ inline SampleKey sample_key(unsigned long long seed, long long row, int step) {
+    const unsigned long long z = splitmix64(seed ^ splitmix64(((unsigned long long)row << 32) | (uint32_t)step));
+    return SampleKey{(uint32_t)z, (uint32_t)(z >> 32)};
+}
+__host__ __device__ inline uint32_t sample_bits(SampleKey k, int word) {
+    uint32_t x = (uint32_t)word ^ k.k0;
+    x ^= x >> 16;
+    x *= 0x7FEB352Du;
+    x ^= x >> 15;
+    x += k.k1;
+    x *= 0x846CA68Bu;
+    x ^= x >> 16;
+    return x;
+}
+#ifdef __CUDACC__
+// g = -log(e), e = -log(u) ~ Exp(1), in fp32 without losing the tail: for u >= 1/2 the complement w = 1 - u =
+// (~bits + 0.5) * 2^-32 is formed exactly and e = -log1p(-w) — its series for w < 1/16 (relative error < 1e-8) — so
+// the largest draws keep their 32-bit resolution (g up to 22.9; a float u would stop at 16.6).  Two fast logarithms
+// (MUFU; absolute error ~4e-7 near 1, relative ~3 ulp elsewhere) and a short polynomial per draw, branch free: this
+// runs once per logit in the vocabulary layer's epilogue.
+__device__ __forceinline__ float sample_gumbel(uint32_t bits) {
+    const bool top = (bits >> 31) != 0u;
+    const float w = fmaf((float)(top ? ~bits : bits), 2.3283064365386963e-10f, 1.1641532182693481e-10f);  // u, or 1 - u
+    const float l = -__logf(top ? 1.0f - w : w);
+    const float s = w * fmaf(w, fmaf(w, fmaf(w, fmaf(w, fmaf(w, 1.0f / 6, 0.2f), 0.25f), 1.0f / 3), 0.5f), 1.0f);
+    return -__logf(top && w < 0.0625f ? s : l);
+}
+#endif
+
 struct DropSpec {          // seedp == nullptr or *seedp == 0: no dropout
     const unsigned long long* seedp;
     unsigned long long stream;

@@ -3,6 +3,7 @@
 //   top-(beam+1) words per row         base_model.py:215-219
 //   TopN / CaptionData heap updates    base_model.py:222-232, utils/misc.py:38-87
 #include "sat_common.cuh"
+#include "sat_linear.cuh"
 #include "sat_rows.cuh"
 
 namespace sat {
@@ -49,7 +50,9 @@ __device__ __forceinline__ float block_sum(float x, float* sm) {
 // of dynamic shared memory available) and the three passes — arg-max, sum of exponentials, probabilities + top-k
 // — run on that copy in small ROLLED loops (this kernel runs once per step from a cold instruction cache: a
 // fully unrolled register-cached version executed 6 k instructions per warp and was instruction-fetch bound).
-template <bool CACHED>
+// SMP: sampling (RowsParams::sample) — best ranks logit / temperature + Gumbel noise, the draw of the fused vocabulary
+// layer (sat_linear.cu) for the same (seed, row, step, word); m stays the raw row maximum.  An instance of its own.
+template <bool CACHED, bool SMP = false>
 __global__ void __launch_bounds__(kRowThreads) rows_softmax_kernel(const RowsParams p) {
     extern __shared__ __align__(16) float row_s[];
     __shared__ ValIdx sm_vi[kRowThreads / 32];
@@ -60,6 +63,44 @@ __global__ void __launch_bounds__(kRowThreads) rows_softmax_kernel(const RowsPar
     const float4* src4 = CACHED ? reinterpret_cast<const float4*>(row_s) : reinterpret_cast<const float4*>(x);
 
     ValIdx best = {-INFINITY, 0x7fffffff};
+    if constexpr (SMP) {
+        const SampleKey sk = sample_key(p.sample->seed, row, p.step);
+        const float itau = p.sample->inv_tau;
+        float mr = -INFINITY;
+        auto offer = [&](float v, int i) {
+            mr = fmaxf(mr, v);
+            const float g = fmaf(v, itau, sample_gumbel(sample_bits(sk, i)));
+            if (better(g, i, best.v, best.i)) { best.v = g; best.i = i; }
+        };
+        if (CACHED) {
+            const float4* x4 = reinterpret_cast<const float4*>(x);
+            float4* d4 = reinterpret_cast<float4*>(row_s);
+#pragma unroll 1
+            for (int i4 = threadIdx.x; i4 < n4; i4 += kRowThreads) {
+                const float4 v = x4[i4];
+                d4[i4] = v;
+                offer(v.x, 4 * i4); offer(v.y, 4 * i4 + 1); offer(v.z, 4 * i4 + 2); offer(v.w, 4 * i4 + 3);
+            }
+        } else {
+#pragma unroll 1
+            for (int i = threadIdx.x; i < V; i += kRowThreads) offer(x[i], i);
+        }
+        best = block_best(best, sm_vi);
+        const ValIdx mx = block_best(ValIdx{mr, 0}, sm_vi);
+        if (threadIdx.x == 0) {
+            if (p.tokens) p.tokens[(size_t)row * p.tokens_ld + p.step] = best.i;
+            if (p.next_word) p.next_word[row] = best.i;
+        }
+        if (!p.word_probs) return;
+        const float m = mx.v;
+        float s = 0.f;
+#pragma unroll 1
+        for (int i = threadIdx.x; i < V; i += kRowThreads) s += expf((CACHED ? row_s[i] : x[i]) - m);
+        s = block_sum(s, sm_f);
+        if (threadIdx.x == 0)   // (a row of NaN logits picks no word: probability 0, no read past the row)
+            p.word_probs[(size_t)row * p.tokens_ld + p.step] = (best.i >= 0 && best.i < V) ? expf(x[best.i] - m) / s : 0.f;
+        return;
+    }
     if (CACHED) {
         const float4* x4 = reinterpret_cast<const float4*>(x);
         float4* d4 = reinterpret_cast<float4*>(row_s);
@@ -166,6 +207,22 @@ cudaError_t rows_softmax_launch(const RowsParams& p, int rows, cudaStream_t st) 
     if (p.topk > kMaxTopK) return cudaErrorInvalidValue;
     const size_t bytes = (size_t)p.V * sizeof(float);
     const bool cached = (p.V % 4) == 0 && bytes <= 96 * 1024 && (reinterpret_cast<uintptr_t>(p.logits) % 16) == 0;
+    if (p.sample) {
+        if (p.forced || p.topk || p.probs || p.argmax) return cudaErrorInvalidValue;
+        if (cached) {
+            static bool smp_attr_set = false;
+            if (!smp_attr_set) {
+                cudaError_t e = cudaFuncSetAttribute(rows_softmax_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                     96 * 1024);
+                if (e != cudaSuccess) return e;
+                smp_attr_set = true;
+            }
+            rows_softmax_kernel<true, true><<<rows, kRowThreads, bytes, st>>>(p);
+        } else {
+            rows_softmax_kernel<false, true><<<rows, kRowThreads, 0, st>>>(p);
+        }
+        return cudaGetLastError();
+    }
     if (cached) {
         static bool attr_set = false;
         if (!attr_set) {
@@ -420,5 +477,39 @@ cudaError_t beam_maps_launch(const BeamParams& p, cudaStream_t st) {
 }
 
 size_t beam_citem_bytes() { return sizeof(CItem); }
+
+// ---------------------------------------------------------------- sampling loop
+__global__ void sample_params_kernel(SampleParams* dst, unsigned long long seed, float inv_tau) {
+    dst->seed = seed;
+    dst->inv_tau = inv_tau;
+    dst->pad = 0.f;
+}
+
+cudaError_t sample_params_launch(SampleParams* dst, unsigned long long seed, float inv_tau, cudaStream_t st) {
+    sample_params_kernel<<<1, 1, 0, st>>>(dst, seed, inv_tau);
+    return cudaGetLastError();
+}
+
+__global__ void __launch_bounds__(256) bcast_state_kernel(const float4* c_src, const float4* h_src, float4* c_dst,
+                                                          float4* h_dst, int rows, int G, int H4) {
+    const long long n = (long long)rows * H4;
+    for (long long i = blockIdx.x * 256ll + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        const long long r = i / H4, q = i - r * H4;
+        const long long s = (r / G) * H4 + q;
+        c_dst[i] = c_src[s];
+        h_dst[i] = h_src[s];
+    }
+}
+
+cudaError_t bcast_state_launch(const float* c_src, const float* h_src, float* c_dst, float* h_dst, int rows, int G, int H,
+                               cudaStream_t st) {
+    if (G < 1 || H % 4) return cudaErrorInvalidValue;
+    const long long n = (long long)rows * (H / 4);
+    int grid = (int)((n + 255) / 256);
+    if (grid > 1024) grid = 1024;
+    bcast_state_kernel<<<grid < 1 ? 1 : grid, 256, 0, st>>>(reinterpret_cast<const float4*>(c_src), reinterpret_cast<const float4*>(h_src),
+                                                       reinterpret_cast<float4*>(c_dst), reinterpret_cast<float4*>(h_dst), rows, G, H / 4);
+    return cudaGetLastError();
+}
 
 }  // namespace sat

@@ -5,6 +5,8 @@
 
 namespace sat {
 
+struct SampleParams;   // sat_linear.cuh
+
 constexpr int kMaxTopK = 8;
 constexpr int kMaxBeam = 7;
 
@@ -24,6 +26,9 @@ struct RowsParams {
     float* topk_p;        // [rows, topk]
     float* word_probs;    // [rows, tokens_ld] or null: word_probs[row, step] = softmax[next word]
                           // (0 for a forced word outside [0, V))
+    const SampleParams* sample;   // sampling loop (no forced words, no top-k): the word is the arg-max of
+                                  // logit / temperature + the Gumbel noise of (seed, row, step, word), as in the fused
+                                  // vocabulary layer; word_probs stay softmax(logits) at temperature 1
 };
 
 struct PItem;
@@ -67,5 +72,10 @@ cudaError_t beam_update_launch(const BeamParams& p, cudaStream_t st);
 cudaError_t beam_finalize_launch(const BeamParams& p, cudaStream_t st);
 cudaError_t beam_maps_launch(const BeamParams& p, cudaStream_t st);   // after finalize, when res_alpha / res_probs
 size_t beam_citem_bytes();
+// sampling loop: *dst = {seed, inv_tau} (one thread, queued on the caller's stream ahead of a replayed graph)
+cudaError_t sample_params_launch(SampleParams* dst, unsigned long long seed, float inv_tau, cudaStream_t st);
+// rows [r] of c_dst / h_dst = rows [r / G] of c_src / h_src ([rows / G, H] -> [rows, H], H % 4 == 0)
+cudaError_t bcast_state_launch(const float* c_src, const float* h_src, float* c_dst, float* h_dst, int rows, int G, int H,
+                               cudaStream_t st);
 
 }  // namespace sat

@@ -11,6 +11,7 @@ Mapping to the reference (SURVEY.md §8b):
   .beam_search(contexts, ...) -> per image list of CaptionData(sentence, score)
                                                    base_model.py:163-240
   .decode_loop(contexts, T, forced_words)          the unrolled loop of model.py:258-312 (greedy / teacher forced)
+  .sample(contexts, num_samples, temperature)      the same loop with each word drawn from softmax(logits / temperature)
 The one intentional deviation: precomputed contexts (conv features) take the place of
 image files, because the CNN is out of scope.  `sess` arguments are accepted and ignored.
 
@@ -102,6 +103,7 @@ class CaptionGenerator(object):
             self.stream = torch.cuda.Stream(self.device, priority=-1)
         self._shapes = weight_shapes(config)
         self._keep = {}
+        self._sample_calls = 0   # seeds of sample(seed=None): a fresh instance repeats its sequence
 
     # ------------------------------------------------------------------ plumbing
     def __del__(self):
@@ -545,6 +547,76 @@ class CaptionGenerator(object):
         self._sync_out()
         self._keep["beam"] = (contexts, sent, lens, scores, nres, comp)
         return sent, lens, scores, nres, comp
+
+    def _sample_seed(self, seed):
+        """seed=None: the next seed of this instance's counter (successive calls differ, a fresh instance repeats)."""
+        if seed is not None:
+            return int(seed) & 0xFFFFFFFFFFFFFFFF
+        self._sample_calls += 1
+        return (self._sample_calls * 0x9E3779B97F4A7C15) & 0xFFFFFFFFFFFFFFFF
+
+    # rows of one image per sat_sample_loop call (the attention kernels share an image's contexts between at most 4)
+    SAMPLE_GROUP = 4
+
+    def sample_device(self, contexts, num_samples, num_steps, temperature=1.0, seed=None, want_word_probs=True):
+        """sat_sample_loop: num_samples captions per image drawn from softmax(logits / temperature).  contexts: CUDA
+        tensor [n, L, D].  Returns tokens [n, K, T] int32 and word_probs [n, K, T] (softmax(logits)[word] at
+        temperature 1) or None (persistent buffers, overwritten by the next call of the same kind).
+        More than SAMPLE_GROUP samples are drawn in groups of SAMPLE_GROUP per image: group c (samples 4c .. 4c+3) is
+        a library call with seed + c * 0x9E3779B97F4A7C15 (mod 2^64), so group 0 is what a call with K <= 4 draws."""
+        torch = self.torch
+        n, K, T = contexts.shape[0], int(num_samples), int(num_steps)
+        if K < 1:
+            raise ValueError("num_samples must be >= 1")
+        seed = self._sample_seed(seed)
+        G = self.SAMPLE_GROUP
+        parts = []
+        self._sync_in()
+        for c in range((K + G - 1) // G):
+            kc = min(G, K - c * G)
+            tokens = self._buf("s_tokens%d" % c, (n, kc, T), torch.int32)
+            wprobs = self._buf("s_word_probs%d" % c, (n, kc, T), torch.float32) if want_word_probs else None
+            sc = (seed + c * 0x9E3779B97F4A7C15) & 0xFFFFFFFFFFFFFFFF
+            self._check(self.lib.sat_sample_loop(self._h, self._p(contexts), n, kc, T, float(temperature), sc,
+                                                 self._p(tokens), self._p(wprobs), self._st()))
+            parts.append((tokens, wprobs))
+        if len(parts) > 1:   # (on our stream: the concatenation is ordered after every group)
+            with torch.cuda.stream(self.stream):
+                tokens = torch.cat([t for t, _ in parts], 1)
+                wprobs = torch.cat([p for _, p in parts], 1) if want_word_probs else None
+        else:
+            tokens, wprobs = parts[0]
+        self._sync_out()
+        self._keep["sample"] = (contexts, tokens, wprobs, parts)
+        return tokens, wprobs
+
+    def sample(self, contexts, num_samples=1, temperature=1.0, seed=None, num_steps=None, eos_id=None):
+        """Sampled captions: per image, num_samples CaptionData drawn word by word from softmax(logits / temperature).
+        sentence: the words up to and including the first eos_id (default config.eos_id), or all num_steps words;
+        complete: whether the caption reached eos_id; word_probs: the model's probability (temperature 1) of each of
+        those words; score: their fp64 product (beam search's convention).  seed: a given seed reproduces the call bit
+        for bit; None draws the next seed of this instance.  contexts: numpy or torch."""
+        cfg = self.config
+        T = int(num_steps or cfg.max_caption_length)
+        eos = int(cfg.eos_id if eos_id is None else eos_id)
+        ctx = self._dev(contexts, self.torch.float32)
+        tokens, wprobs = self.sample_device(ctx, num_samples, T, temperature, seed)
+        self.torch.cuda.synchronize(self.device)
+        tokens, wprobs = tokens.cpu().numpy(), wprobs.cpu().numpy()
+        results = []
+        for k in range(tokens.shape[0]):
+            caps = []
+            for j in range(tokens.shape[1]):
+                row = tokens[k, j]
+                hit = np.flatnonzero(row == eos)
+                ln = int(hit[0]) + 1 if hit.size else T
+                wp = wprobs[k, j, :ln].copy()
+                score = 1.0
+                for x in wp:
+                    score *= float(x)
+                caps.append(CaptionData([int(w) for w in row[:ln]], score, bool(hit.size), word_probs=wp))
+            results.append(caps)
+        return results
 
     # ------------------------------------------------------------------ reference-shaped API
     def initialize(self, contexts, sess=None):
