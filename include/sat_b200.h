@@ -257,6 +257,31 @@ int sat_train_forward_backward(sat_handle* h, const float* params, float* grads,
 int sat_train_forward_backward_dsum(sat_handle* h, const float* params, float* grads, const float* contexts,
                                     const int32_t* sentences, const float* masks, int32_t B, int32_t T, uint64_t seed,
                                     const double* global_mask_sum_dev, int32_t global_batch, float* losses, void* stream);
+/* Grouped training step: several captions per image (sampled captions for self-critical training, or the reference
+ * captions of an image) with the image's contexts shared by its rows instead of replicated.
+ * rows = n_img * group; row r is a caption of image r / group.  sat_train_init(h, B, T, ...) ==
+ * sat_train_init_grouped(h, B, 1, T, ...).  What depends on the image alone (context mean, initialize, attend/fc_1a and
+ * its stash) is computed once per image, with the init_* and att_ctx dropout masks drawn for n_img rows (n_img * L for
+ * att_ctx); every other mask is drawn per row.  The tensor-core attend/fc_1a path needs n_img * L % 128 == 0. */
+int sat_train_init_grouped(sat_handle* h, int32_t n_img, int32_t group, int32_t T, float fc_drop_rate,
+                           float lstm_drop_rate, float attention_loss_factor, float fc_kernel_regularizer_scale);
+/* contexts [n_img, L, D]; sentences / masks [rows, T]; row_weights [rows] or NULL (= 1): row r's cross entropy and its
+ * gradient are multiplied by row_weights[r] (e.g. a policy-gradient advantage, any sign; read on the device at run time,
+ * so new values in the same buffer replay the captured graph).  Accuracy and the attention loss are not weighted.
+ * global_batch counts rows (coverage normaliser); losses[0] = sum_r w_r sum_t m_rt CE_rt / global mask sum.
+ * sat_train_forward_backward(_dsum) compute the same with group 1 and NULL weights.
+ * Errors: SAT_ERR_INVALID, with nothing enqueued, for group < 1, an (n_img, group, T) other than the one of
+ * sat_train_init_grouped, or a null required argument; the values in row_weights are not checked. */
+int sat_train_forward_backward_grouped(sat_handle* h, const float* params, float* grads, const float* contexts,
+                                       int32_t n_img, int32_t group, const int32_t* sentences, const float* masks,
+                                       const float* row_weights, int32_t T, uint64_t seed,
+                                       const double* global_mask_sum_dev, int32_t global_batch, float* losses,
+                                       void* stream);
+/* caption masks of token rows (e.g. sat_sample_loop's output), on the device: masks[r, t] = 1 for t <= the first t'
+ * with tokens[r, t'] == eos_id (all T if there is none), else 0; *mask_sum (device double, may be NULL) = their sum.
+ * Needs no handle: runs on the current device.  SAT_ERR_INVALID for null tokens / masks, rows < 0 or T < 1. */
+int sat_caption_masks(const int32_t* tokens, int32_t rows, int32_t T, int32_t eos_id, float* masks,
+                      double* mask_sum, void* stream);
 /* adds the L2-regulariser gradient, clips by the global norm (clip_gradients, config.py:36) and applies TF Adam
  * (config.py:32-43).  step counts from 1.  grad_norm (device, 1 float, may be NULL) receives the squared norm. */
 int sat_train_apply(sat_handle* h, float* params, float* grads, float* adam_m, float* adam_v, int64_t step, float lr,

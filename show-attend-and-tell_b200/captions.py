@@ -114,3 +114,38 @@ def write_attention_maps(path, image_files, captions, vocabulary):
         out["img%d_alphas" % i] = alphas
     np.savez(path, **out)
     return path
+
+
+def cut_after_eos(tokens, eos_id):
+    """Word ids of one caption up to and including the first eos_id (all of them if there is none)."""
+    ids = [int(w) for w in tokens]
+    return ids[:ids.index(int(eos_id)) + 1] if int(eos_id) in ids else ids
+
+
+def scst_advantages(rewards, num_samples, baseline="greedy"):
+    """Self-critical advantages of K sampled captions per image (pure host arithmetic, float64).
+
+    rewards: [n, K + 1] for baseline "greedy" (column K is the reward of the image's greedy caption), [n, K] for
+    baseline "mean" (each sample's baseline is the mean reward of the image's OTHER K - 1 samples, so K >= 2).
+    Returns (advantages [n, K] = sample reward - baseline, mean sample reward, mean baseline reward)."""
+    import numpy as np
+    K = int(num_samples)
+    r = np.asarray(rewards, dtype=np.float64)
+    if K < 1:
+        raise ValueError("num_samples must be >= 1")
+    if baseline == "greedy":
+        if r.ndim != 2 or r.shape[1] != K + 1:
+            raise ValueError("baseline 'greedy': rewards must be [n, %d] (K samples, then the greedy caption), got %s"
+                             % (K + 1, r.shape))
+        samples = r[:, :K]
+        base = np.broadcast_to(r[:, K:], samples.shape)
+    elif baseline == "mean":
+        if K < 2:
+            raise ValueError("baseline 'mean' (leave-one-out) needs num_samples >= 2")
+        if r.ndim != 2 or r.shape[1] != K:
+            raise ValueError("baseline 'mean': rewards must be [n, %d], got %s" % (K, r.shape))
+        samples = r
+        base = (r.sum(axis=1, keepdims=True) - r) / (K - 1)
+    else:
+        raise ValueError("baseline must be 'greedy' or 'mean', got %r" % (baseline,))
+    return samples - base, float(samples.mean()), float(base.mean())

@@ -478,16 +478,18 @@ __global__ void att_temp_kernel(float* temp, const float* T1, const float* q, in
 }
 // e[b*L + l] = sum_a (T1[b*L + l, a] + q[b, a]) * drop(att_mid) * w2[a]: att_temp + rowdot in one pass over T1 (temp is
 // not stored; the backward pass rebuilds it from T1, q and the mask).  One warp per row, A % 4 == 0.
+// group > 1: T1 holds one [L, A] block per image and batch row b reads the block of image b / group
 __global__ void att_logits_kernel(float* __restrict__ e, const float* __restrict__ T1, const float* __restrict__ q,
                                   const float* __restrict__ w2, int B, int L, int A,
-                                  const unsigned long long* seedp, unsigned long long stream, float keep) {
+                                  const unsigned long long* seedp, unsigned long long stream, float keep, int group = 1) {
     pdl_enter();
     const unsigned long long seed = *seedp;
     const DropGen gen = drop_gen(seed, stream, keep);
     const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (row >= B * L) return;
     const int A4 = A >> 2, b = row / L;
-    const float4* t4 = reinterpret_cast<const float4*>(T1) + (size_t)row * A4;
+    const int trow = group == 1 ? row : (b / group) * L + (row - b * L);
+    const float4* t4 = reinterpret_cast<const float4*>(T1) + (size_t)trow * A4;
     const float4* q4 = reinterpret_cast<const float4*>(q) + (size_t)b * A4;
     const float4* w4 = reinterpret_cast<const float4*>(w2);
     float s = 0.f;
@@ -598,6 +600,138 @@ __global__ void __launch_bounds__(kAbRG* kAbCT, 4) att_bwd_fused_wave_kernel(ATT
     att_bwd_fused_body(dtemp, dq, dw2, db, T1, q, de, w2, L, A, chunk_rows, seedp, stream, keep, alpha);
 }
 #undef ATT_BWD_ARGS
+// The same backward pass when the rows of an image share its T1 block (rows b = img * group + k, k < group; T1 and
+// dtemp hold one [L, A] block per image).  Each (l, column) of the image's T1 chunk is read once per tile of kAbGT rows:
+//   dtemp[img, l, a] = sum_k de[b, l] * w2[a] * m[b, l, a] * (1 - T1[img, l, a]^2)     (summed over the group)
+//   dq[b, a] += sum_l de[b, l] * w2[a] * m[b, l, a]  per row; dw2 and db as above
+// grid (ceil(A/256), row chunks, n_img); att_mid masks stay per row (index (b * L + l) * A + a, as in att_logits_kernel).
+constexpr int kAbGT = kAbRG * kAbCT / 32;   // rows per tile: one warp computes the softmax dot product of one row
+__global__ void __launch_bounds__(kAbRG* kAbCT) att_bwd_grouped_kernel(
+    float* __restrict__ dtemp, float* dq, float* dw2, float* db, const float* __restrict__ T1, const float* __restrict__ q,
+    const float* __restrict__ de, const float* __restrict__ w2, int L, int A, int chunk_rows, int group,
+    const unsigned long long* seedp, unsigned long long stream, float keep, const float* __restrict__ alpha) {
+    pdl_enter();
+    __shared__ float4 red[kAbRG - 1][kAbCT];
+    __shared__ float sd[kAbGT];
+    const unsigned long long seed = *seedp;
+    const DropGen gen = drop_gen(seed, stream, keep);
+    const int ct = threadIdx.x % kAbCT, rg = threadIdx.x / kAbCT, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int A4 = A >> 2, c4 = blockIdx.x * kAbCT + ct, img = blockIdx.z;
+    const int l0 = blockIdx.y * chunk_rows, l1 = min(L, l0 + chunk_rows);
+    const bool on = c4 < A4;
+    const float4 w = on ? reinterpret_cast<const float4*>(w2)[c4] : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 aw = make_float4(0.f, 0.f, 0.f, 0.f), ab = aw;
+    // sum of a float4 over the kAbRG row groups, left in row group 0
+    auto reduce_rg = [&](float4 v) -> float4 {
+        __syncthreads();
+        if (rg > 0) red[rg - 1][ct] = v;
+        __syncthreads();
+        if (rg == 0) {
+#pragma unroll
+            for (int g = 0; g < kAbRG - 1; ++g) {
+                const float4 x = red[g][ct];
+                v.x += x.x; v.y += x.y; v.z += x.z; v.w += x.w;
+            }
+        }
+        return v;
+    };
+    for (int k0 = 0; k0 < group; k0 += kAbGT) {
+        const int kn = min(kAbGT, group - k0);
+        const size_t b0 = (size_t)img * group + k0;   // first batch row of this tile
+        if (alpha) {   // softmax backward folded in: sd[j] = sum_l alpha[b, l] * dalpha[b, l] of row b0 + j
+            __syncthreads();
+            if (warp < kn) {
+                float p = 0.f;
+                for (int l = lane; l < L; l += 32) p = fmaf(alpha[(b0 + warp) * L + l], de[(b0 + warp) * L + l], p);
+                for (int o = 16; o > 0; o >>= 1) p += __shfl_xor_sync(0xffffffffu, p, o);
+                if (lane == 0) sd[warp] = p;
+            }
+            __syncthreads();
+        }
+        float4 aq[kAbGT];
+#pragma unroll
+        for (int j = 0; j < kAbGT; ++j) aq[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (on) {
+            for (int l = l0 + rg; l < l1; l += kAbRG) {
+                const size_t ti = ((size_t)img * L + l) * A4 + c4;
+                const float4 t = reinterpret_cast<const float4*>(T1)[ti];
+                float4 gs = make_float4(0.f, 0.f, 0.f, 0.f);   // sum over the tile's rows of d temp
+#pragma unroll
+                for (int j = 0; j < kAbGT; ++j) {
+                    if (j < kn) {
+                        const size_t r = (b0 + j) * L + l;
+                        const float d = alpha ? alpha[r] * (de[r] - sd[j]) : de[r];
+                        const float4 qq = reinterpret_cast<const float4*>(q)[(b0 + j) * A4 + c4];
+                        float4 m = make_float4(1.f, 1.f, 1.f, 1.f);
+                        if (seed) {
+                            const unsigned long long i = (r * A4 + c4) << 2;
+                            m.x = gen.scale(i);
+                            m.y = gen.scale(i + 1);
+                            m.z = gen.scale(i + 2);
+                            m.w = gen.scale(i + 3);
+                        }
+                        const float4 dm = make_float4(d * m.x, d * m.y, d * m.z, d * m.w);
+                        const float4 g = make_float4(dm.x * w.x, dm.y * w.y, dm.z * w.z, dm.w * w.w);
+                        aq[j].x += g.x; aq[j].y += g.y; aq[j].z += g.z; aq[j].w += g.w;
+                        gs.x += g.x; gs.y += g.y; gs.z += g.z; gs.w += g.w;
+                        aw.x = fmaf(t.x + qq.x, dm.x, aw.x); aw.y = fmaf(t.y + qq.y, dm.y, aw.y);
+                        aw.z = fmaf(t.z + qq.z, dm.z, aw.z); aw.w = fmaf(t.w + qq.w, dm.w, aw.w);
+                    }
+                }
+                float4 o = make_float4(gs.x * (1.0f - t.x * t.x), gs.y * (1.0f - t.y * t.y), gs.z * (1.0f - t.z * t.z),
+                                       gs.w * (1.0f - t.w * t.w));
+                ab.x += o.x; ab.y += o.y; ab.z += o.z; ab.w += o.w;
+                float4* pd = reinterpret_cast<float4*>(dtemp) + ti;
+                if (k0) {   // (the same thread wrote this element for the previous tile)
+                    const float4 p = *pd;
+                    o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w;
+                }
+                *pd = o;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < kAbGT; ++j) {
+            if (j < kn) {
+                const float4 v = reduce_rg(aq[j]);
+                if (rg == 0 && on) {
+                    float* pq = dq + ((b0 + j) * A4 + c4) * 4;
+                    atomicAdd(pq, v.x); atomicAdd(pq + 1, v.y); atomicAdd(pq + 2, v.z); atomicAdd(pq + 3, v.w);
+                }
+            }
+        }
+    }
+    aw = reduce_rg(aw);
+    ab = reduce_rg(ab);
+    if (rg == 0 && on) {
+        float* pw = dw2 + (size_t)c4 * 4;
+        atomicAdd(pw, aw.x); atomicAdd(pw + 1, aw.y); atomicAdd(pw + 2, aw.z); atomicAdd(pw + 3, aw.w);
+        if (db) {
+            float* pb = db + (size_t)c4 * 4;
+            atomicAdd(pb, ab.x); atomicAdd(pb + 1, ab.y); atomicAdd(pb + 2, ab.z); atomicAdd(pb + 3, ab.w);
+        }
+    }
+}
+// y[r, c] = x[r / group, c] for r < rows: image-level rows copied to each of the image's batch rows
+__global__ void expand_rows_kernel(float* __restrict__ y, const float* __restrict__ x, int rows, int cols, int group) {
+    pdl_enter();
+    const size_t n = (size_t)rows * cols;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t r = i / cols, c = i - r * cols;
+        y[i] = x[(r / group) * cols + c];
+    }
+}
+// y[i, c] = sum_k x[i * group + k, c] for i < n_img: the transpose of expand_rows_kernel
+__global__ void group_sum_kernel(float* __restrict__ y, const float* __restrict__ x, int n_img, int cols, int group) {
+    pdl_enter();
+    const size_t n = (size_t)n_img * cols;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t r = i / cols, c = i - r * cols;
+        const float* p = x + r * group * cols + c;
+        float s = 0.f;
+        for (int k = 0; k < group; ++k) s += p[(size_t)k * cols];
+        y[i] = s;
+    }
+}
 // e[r] = sum_a temp[r, a] * w2[a]       (one warp per row)
 __global__ void rowdot_kernel(float* e, const float* temp, const float* w2, int rows, int A) {
     pdl_enter();
@@ -641,12 +775,12 @@ __global__ void softmax_bwd_kernel(float* dalpha, const float* alpha, int rows, 
         dalpha[i] = alpha[i] * (dalpha[i] - s);
     }
 }
-// z[b, d] = sum_l alpha[b, l] * ctx[b, l, d]
-__global__ void context_fwd_kernel(float* z, const float* alpha, const float* ctx, int B, int L, int D) {
+// z[b, d] = sum_l alpha[b, l] * ctx[b / group, l, d]  (group > 1: the rows of an image share its contexts; likewise below)
+__global__ void context_fwd_kernel(float* z, const float* alpha, const float* ctx, int B, int L, int D, int group = 1) {
     pdl_enter();
     const int b = blockIdx.y, d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= D) return;
-    const float* c = ctx + (size_t)b * L * D + d;
+    const float* c = ctx + (size_t)(b / group) * L * D + d;
     float s = 0.f;
     for (int l = 0; l < L; ++l) s = fmaf(alpha[(size_t)b * L + l], c[(size_t)l * D], s);
     z[(size_t)b * D + d] = s;
@@ -654,14 +788,14 @@ __global__ void context_fwd_kernel(float* z, const float* alpha, const float* ct
 // the same on float4 columns with eight rows in flight per column: grid (ceil(D / 128), B), 256 threads =
 // 8 row groups x 32 float4 columns, row groups summed through shared memory (D % 4 == 0, 16-byte aligned)
 __global__ void __launch_bounds__(256) context_fwd4_kernel(float* __restrict__ z, const float* __restrict__ alpha,
-                                                            const float* __restrict__ ctx, int L, int D) {
+                                                            const float* __restrict__ ctx, int L, int D, int group = 1) {
     pdl_enter();
     __shared__ float4 red[7][32];
     const int ct = threadIdx.x & 31, rg = threadIdx.x >> 5, b = blockIdx.y;
     const int D4 = D >> 2, c4 = blockIdx.x * 32 + ct;
     float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
     if (c4 < D4) {
-        const float4* c = reinterpret_cast<const float4*>(ctx) + (size_t)b * L * D4 + c4;
+        const float4* c = reinterpret_cast<const float4*>(ctx) + (size_t)(b / group) * L * D4 + c4;
         const float* al = alpha + (size_t)b * L;
 #pragma unroll 4
         for (int l = rg; l < L; l += 8) {
@@ -688,7 +822,8 @@ __global__ void __launch_bounds__(256) context_fwd4_kernel(float* __restrict__ z
 constexpr int kSmL = 1024;
 __global__ void __launch_bounds__(256) softmax_context_fwd4_kernel(float* __restrict__ z, float* __restrict__ alpha,
                                                                     const float* __restrict__ e, const float* __restrict__ ctx,
-                                                                    int L, int D, float* att, const float* masks, int mld, int t) {
+                                                                    int L, int D, float* att, const float* masks, int mld, int t,
+                                                                    int group = 1) {
     pdl_enter();
     __shared__ float4 red[7][32];
     __shared__ float al_s[kSmL];
@@ -729,7 +864,7 @@ __global__ void __launch_bounds__(256) softmax_context_fwd4_kernel(float* __rest
     const int D4 = D >> 2, c4 = blockIdx.x * 32 + ct;
     float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
     if (c4 < D4) {
-        const float4* c = reinterpret_cast<const float4*>(ctx) + (size_t)b * L * D4 + c4;
+        const float4* c = reinterpret_cast<const float4*>(ctx) + (size_t)(b / group) * L * D4 + c4;
 #pragma unroll 4
         for (int l = rg; l < L; l += 8) {
             const float4 v = c[(size_t)l * D4];
@@ -750,13 +885,14 @@ __global__ void __launch_bounds__(256) softmax_context_fwd4_kernel(float* __rest
 }
 // dalpha[b, l] = sum_d dz[b, d] * ctx[b, l, d]  (+ extra[b, l] * mask[b, t] if given)   (one warp per (b, l))
 __global__ void context_bwd_kernel(float* dalpha, const float* dz, const float* ctx, const float* extra, int B, int L, int D,
-                                   const float* masks, int mld, int t) {
+                                   const float* masks, int mld, int t, int group = 1) {
     pdl_enter();
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= B * L) return;
     const int b = warp / L;
+    const size_t crow = group == 1 ? (size_t)warp : (size_t)(b / group) * L + (warp - b * L);
     float s = 0.f;
-    for (int d = lane; d < D; d += 32) s = fmaf(dz[(size_t)b * D + d], ctx[(size_t)warp * D + d], s);
+    for (int d = lane; d < D; d += 32) s = fmaf(dz[(size_t)b * D + d], ctx[crow * D + d], s);
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     // extra = d coverage loss / d att (datt); it reaches alpha[b, l] of step t through att += alpha * mask[b, t]
     if (lane == 0) dalpha[warp] = s + (extra ? extra[warp] * masks[(size_t)b * mld + t] : 0.f);
@@ -859,9 +995,12 @@ __global__ void lstm_bwd_kernel(float* dG, float* dc, const float* dh_out, const
 // masked cross entropy of one time step + its gradient; one block per row
 constexpr int kCeThreads = 1024;   // one CTA per batch row: the three passes over the V logits are latency bound
 // (rows_per_step > 0: block r is row r % rows_per_step of time step t + r / rows_per_step — all T steps in one launch)
+// kWeighted: the gradient and the cross entropy of row b are scaled by row_w[b] (a policy-gradient advantage, any sign);
+// the accuracy is not
+template <bool kWeighted>
 __global__ void __launch_bounds__(kCeThreads) ce_kernel(const float* logits, float* dlogits, const int32_t* sent, int sent_ld, int t,
                                                         const float* masks, int V, const float* inv_msum_p, float* loss_acc,
-                                                        int rows_per_step) {
+                                                        int rows_per_step, const float* row_w) {
     pdl_enter();
     constexpr int NW = kCeThreads / 32;
     const float inv_msum = *inv_msum_p;
@@ -904,7 +1043,7 @@ __global__ void __launch_bounds__(kCeThreads) ce_kernel(const float* logits, flo
     const bool y_ok = (unsigned)y_raw < (unsigned)V;      // (an id outside the vocabulary: no target, counted as bad)
     const int y = y_ok ? y_raw : 0;
     const float mk = y_ok ? masks[(size_t)b * sent_ld + t] : 0.f;
-    const float scale = mk * inv_msum;
+    const float scale = kWeighted ? mk * inv_msum * row_w[b] : mk * inv_msum;
     for (int i = threadIdx.x; i < V; i += kCeThreads) {
         const float p = d[i] / s;
         d[i] = (p - (i == y ? 1.0f : 0.0f)) * scale;
@@ -1049,6 +1188,11 @@ const char* kVarNames[kNumVars] = {
 struct TrainState {
     sat_dims d;
     int B = 0, T = 0;
+    // B = n_img * group batch rows; row r is a caption of image r / group.  What depends on the image alone (context
+    // mean, initialize, attend/fc_1a and its T1 stash) is computed on n_img rows, the rest on B rows.
+    int n_img = 0, group = 1;
+    float *c0i = nullptr, *h0i = nullptr, *dci = nullptr, *dhi = nullptr;   // group > 1: image-level c0 / h0 and gradients
+    float *e_img = nullptr, *dtemp_g = nullptr;   // group > 1: 1-layer image scores / group-summed d temp (non-fused scorer)
     float keep_fc = 0.5f, keep_lstm = 0.7f, att_factor = 0.01f, reg_scale = 1e-4f;
     size_t off[kNumVars + 1];
     int rows[kNumVars], cols[kNumVars];
@@ -1182,13 +1326,14 @@ extern "C" int sat_train_num_vars(sat_handle* h) {
     return tmp.num_present;
 }
 
-extern "C" int sat_train_init(sat_handle* h, int32_t B, int32_t T, float fc_drop_rate, float lstm_drop_rate,
-                              float attention_loss_factor, float fc_kernel_regularizer_scale) {
+extern "C" int sat_train_init_grouped(sat_handle* h, int32_t n_img, int32_t group, int32_t T, float fc_drop_rate,
+                                      float lstm_drop_rate, float attention_loss_factor, float fc_kernel_regularizer_scale) {
     if (!h) return sat_fail(SAT_ERR_INVALID, "null handle");
     const sat_dims* dp = sat_handle_dims(h);
     for (int nl : {dp->num_attend_layers, dp->num_decode_layers, dp->num_initalize_layers})
         if (nl != 1 && nl != 2) return sat_fail(SAT_ERR_UNSUPPORTED, "attend/decode/initialize have 1 or 2 layers (got %d)", nl);
-    if (B < 1 || T < 1) return sat_fail(SAT_ERR_INVALID, "bad B/T");
+    if (n_img < 1 || group < 1 || T < 1 || (int64_t)n_img * group > INT32_MAX) return sat_fail(SAT_ERR_INVALID, "bad B/T");
+    const int32_t B = n_img * group;
     TCK(cudaSetDevice(sat_handle_device(h)));
     void** slot = sat_handle_train_slot(h);
     if (*slot) { train_free(*slot); *slot = nullptr; }
@@ -1196,6 +1341,8 @@ extern "C" int sat_train_init(sat_handle* h, int32_t B, int32_t T, float fc_drop
     s->d = *dp;
     s->B = B;
     s->T = T;
+    s->n_img = n_img;
+    s->group = group;
     s->keep_fc = (float)(1.0 - (double)fc_drop_rate);      // same value as numpy's float32(1 - rate)
     s->keep_lstm = (float)(1.0 - (double)lstm_drop_rate);
     s->att_factor = attention_loss_factor;
@@ -1212,12 +1359,17 @@ extern "C" int sat_train_init(sat_handle* h, int32_t B, int32_t T, float fc_drop
         A1(&base, n * T);
         for (int t = 0; t < T && base; ++t) v[t] = base + (size_t)t * n;
     };
-    AT(s->T1, BL * A); AT(s->q, B * A); AT(s->hd, B * H); AT(s->alpha, B * L); AT(s->z, B * D); AT(s->lstm_in, B * (D + E + H));
+    const size_t NI = (size_t)n_img, BLi = NI * L;   // image-level rows
+    AT(s->T1, BLi * A); AT(s->q, B * A); AT(s->hd, B * H); AT(s->alpha, B * L); AT(s->z, B * D); AT(s->lstm_in, B * (D + E + H));
     AT(s->acts, B * 4 * H); AT(s->c, B * H); AT(s->h_out, B * H); AT(s->h_state, B * H); AT(s->expd, B * (H + D + E));
     AT(s->t1, B * Dd); AT(s->td, B * Dd); AT(s->dlogits, B * V); AT(s->emb, B * E);
-    A1(&s->ctxd, BL * D); A1(&s->temp, BL * A); A1(&s->e, BL); A1(&s->G, B * 4 * H); A1(&s->logits, B * V);
-    A1(&s->mean, B * D); A1(&s->meand, B * D); A1(&s->ia1, B * I); A1(&s->ia1d, B * I); A1(&s->ib1, B * I); A1(&s->ib1d, B * I);
+    A1(&s->ctxd, BLi * D); A1(&s->temp, BL * A); A1(&s->e, BL); A1(&s->G, B * 4 * H); A1(&s->logits, B * V);
+    A1(&s->mean, NI * D); A1(&s->meand, NI * D); A1(&s->ia1, NI * I); A1(&s->ia1d, NI * I); A1(&s->ib1, NI * I); A1(&s->ib1d, NI * I);
     A1(&s->c0, B * H); A1(&s->h0, B * H); A1(&s->att, BL); A1(&s->datt, BL);
+    if (group > 1) {
+        A1(&s->c0i, NI * H); A1(&s->h0i, NI * H); A1(&s->dci, NI * H); A1(&s->dhi, NI * H);
+        A1(&s->e_img, BLi); A1(&s->dtemp_g, BLi * A);
+    }
     A1(&s->dtd, B * Dd); A1(&s->dexp, B * (H + D + E)); A1(&s->dh_out, B * H); A1(&s->dh_state, B * H);
     A1(&s->dc, B * H); A1(&s->dG, B * 4 * H); A1(&s->dlin, B * (D + E + H)); A1(&s->dz, B * D); A1(&s->demb, B * E);
     A1(&s->dalpha, BL); A1(&s->dtemp, BL * A); A1(&s->dq, B * A); A1(&s->dhd, B * H); A1(&s->dbuf, B * (D + E + I + H));
@@ -1225,14 +1377,14 @@ extern "C" int sat_train_init(sat_handle* h, int32_t B, int32_t T, float fc_drop
     A1(&s->demb_all, (size_t)T * B * E);
     s->handle = h;
     const bool att2 = d.num_attend_layers == 2, dec2 = d.num_decode_layers == 2;
-    s->tc_ok = att2 && (D % 128 == 0) && (A % 128 == 0) && (BL % 128 == 0);
+    s->tc_ok = att2 && (D % 128 == 0) && (A % 128 == 0) && (BLi % 128 == 0);
     if (s->tc_ok) {
         float* f = nullptr;   // (sizes in floats: a packed operand takes 4 bytes per element, like fp32)
-        A1(&f, BL * D); s->tc_xpa = reinterpret_cast<uint8_t*>(f);
-        A1(&f, BL * (A > D ? A : D)); s->tc_wbig = reinterpret_cast<uint8_t*>(f);
+        A1(&f, BLi * D); s->tc_xpa = reinterpret_cast<uint8_t*>(f);
+        A1(&f, BLi * (A > D ? A : D)); s->tc_wbig = reinterpret_cast<uint8_t*>(f);
         A1(&f, D * A); s->tc_w1a = reinterpret_cast<uint8_t*>(f);
         A1(&s->tc_b1a, A);
-        A1(&s->dtemp2, BL * A);
+        A1(&s->dtemp2, BLi * A);   // (used by the fused scorer only, which writes image-level d temp)
         int lo_pri = 0, hi_pri = 0;
         cudaDeviceGetStreamPriorityRange(&lo_pri, &hi_pri);
         if (rc == SAT_OK && cudaStreamCreateWithPriority(&s->side, cudaStreamNonBlocking, lo_pri) == cudaSuccess) {
@@ -1320,6 +1472,11 @@ extern "C" int sat_train_init(sat_handle* h, int32_t B, int32_t T, float fc_drop
     return SAT_OK;
 }
 
+extern "C" int sat_train_init(sat_handle* h, int32_t B, int32_t T, float fc_drop_rate, float lstm_drop_rate,
+                              float attention_loss_factor, float fc_kernel_regularizer_scale) {
+    return sat_train_init_grouped(h, B, 1, T, fc_drop_rate, lstm_drop_rate, attention_loss_factor, fc_kernel_regularizer_scale);
+}
+
 int sat_train_info(sat_handle* h, const char* key, int64_t* value, int* rc) {
     if (strcmp(key, "train_bad_ids") != 0) return 0;
     TrainState* s = (TrainState*)*sat_handle_train_slot(h);
@@ -1366,12 +1523,14 @@ static int dense_bwd(cudaStream_t st, const float* x, int rows, int K, const flo
 }
 
 static int train_enqueue(TrainState* s, const float* params, float* grads, const float* contexts,
-                         const int32_t* sentences, const float* masks, int32_t B, int32_t T, int32_t global_batch,
-                         float* losses, cudaStream_t st) {
+                         const int32_t* sentences, const float* masks, const float* row_w, int32_t B, int32_t T,
+                         int32_t global_batch, float* losses, cudaStream_t st) {
     const sat_dims& d = s->d;
     const int L = d.num_ctx, D = d.dim_ctx, E = d.dim_embedding, H = d.num_lstm_units, A = d.dim_attend_layer,
               Dd = d.dim_decode_layer, I = d.dim_initalize_layer, V = d.vocabulary_size;
     const int BL = B * L, XL = D + E + H, XD = H + D + E;
+    // image-level rows: NI images of G batch rows each (G == 1: NI == B, and every launch below is the ungrouped one)
+    const int G = s->group, NI = s->n_img, BLi = NI * L;
     const float kf = s->keep_fc, kl = s->keep_lstm;   // 1 - fc_drop_rate, 1 - lstm_drop_rate (config.py:25-26)
     auto P = [&](int v) { return params + s->off[v]; };
     auto Gd = [&](int v) { return grads + s->off[v]; };
@@ -1386,19 +1545,26 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
     TCK(cudaMemsetAsync(s->att, 0, (size_t)BL * sizeof(float), st));
 
     // ------------------------------------------------------------ initialize (model.py:239-242, 358-393)
-    launch_k(mean_L_kernel, dim3((D + 127) / 128, B), 128, st, s->mean, contexts, L, D);
-    launch_k(dropout2d_kernel, GRID1D((size_t)B * D), 256, st, s->meand, D, s->mean, D, B, D, seed, INIT + 0, kf, 0);
+    // (per image; the init_* masks are drawn for NI rows)
+    float* const c0i = G > 1 ? s->c0i : s->c0;
+    float* const h0i = G > 1 ? s->h0i : s->h0;
+    launch_k(mean_L_kernel, dim3((D + 127) / 128, NI), 128, st, s->mean, contexts, L, D);
+    launch_k(dropout2d_kernel, GRID1D((size_t)NI * D), 256, st, s->meand, D, s->mean, D, NI, D, seed, INIT + 0, kf, 0);
     const bool init2 = d.num_initalize_layers == 2, att2 = d.num_attend_layers == 2, dec2 = d.num_decode_layers == 2;
     if (init2) {
-        TRET(dense_fwd(st, s->meand, B, D, P(vIa1W), P(vIa1B), I, s->ia1, 1));
-        launch_k(dropout2d_kernel, GRID1D((size_t)B * I), 256, st, s->ia1d, I, s->ia1, I, B, I, seed, INIT + 1, kf, 0);
-        TRET(dense_fwd(st, s->ia1d, B, I, P(vIa2W), P(vIa2B), H, s->c0, 0));
-        TRET(dense_fwd(st, s->meand, B, D, P(vIb1W), P(vIb1B), I, s->ib1, 1));
-        launch_k(dropout2d_kernel, GRID1D((size_t)B * I), 256, st, s->ib1d, I, s->ib1, I, B, I, seed, INIT + 2, kf, 0);
-        TRET(dense_fwd(st, s->ib1d, B, I, P(vIb2W), P(vIb2B), H, s->h0, 0));
+        TRET(dense_fwd(st, s->meand, NI, D, P(vIa1W), P(vIa1B), I, s->ia1, 1));
+        launch_k(dropout2d_kernel, GRID1D((size_t)NI * I), 256, st, s->ia1d, I, s->ia1, I, NI, I, seed, INIT + 1, kf, 0);
+        TRET(dense_fwd(st, s->ia1d, NI, I, P(vIa2W), P(vIa2B), H, c0i, 0));
+        TRET(dense_fwd(st, s->meand, NI, D, P(vIb1W), P(vIb1B), I, s->ib1, 1));
+        launch_k(dropout2d_kernel, GRID1D((size_t)NI * I), 256, st, s->ib1d, I, s->ib1, I, NI, I, seed, INIT + 2, kf, 0);
+        TRET(dense_fwd(st, s->ib1d, NI, I, P(vIb2W), P(vIb2B), H, h0i, 0));
     } else {   // one layer each, no activation (model.py:362-371)
-        TRET(dense_fwd(st, s->meand, B, D, P(vIa1W), P(vIa1B), H, s->c0, 0));
-        TRET(dense_fwd(st, s->meand, B, D, P(vIb1W), P(vIb1B), H, s->h0, 0));
+        TRET(dense_fwd(st, s->meand, NI, D, P(vIa1W), P(vIa1B), H, c0i, 0));
+        TRET(dense_fwd(st, s->meand, NI, D, P(vIb1W), P(vIb1B), H, h0i, 0));
+    }
+    if (G > 1) {   // every caption of an image starts from the image's state
+        launch_k(expand_rows_kernel, GRID1D((size_t)B * H), 256, st, s->c0, (const float*)c0i, B, H, G);
+        launch_k(expand_rows_kernel, GRID1D((size_t)B * H), 256, st, s->h0, (const float*)h0i, B, H, G);
     }
 
     const bool tc = s->tc_ok && sat_handle_train_tc(s->handle);
@@ -1497,7 +1663,8 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
     int ab_chunks = 1, ab_rows = L, ab_wave = 0;
     {
         const int gx = (A / 4 + kAbCT - 1) / kAbCT;
-        ab_chunks = (sat::device_sm_count() * 4 + B * gx - 1) / (B * gx > 0 ? B * gx : 1);   // about four CTAs per SM
+        // about four CTAs per SM (grouped: one CTA covers the rows of an image)
+        ab_chunks = (sat::device_sm_count() * 4 + NI * gx - 1) / (NI * gx > 0 ? NI * gx : 1);
         if (ab_chunks > (L + 15) / 16) ab_chunks = (L + 15) / 16;
         if (ab_chunks < 1) ab_chunks = 1;
         // SAT_TRAIN_ATTBWD_WAVE=1 (experiment, off by default): the 64-register build of the kernel and as many row
@@ -1509,42 +1676,58 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
             cudaGetDevice(&dev);
             cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
             if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, att_bwd_fused_wave_kernel, kAbRG * kAbCT, 0) != cudaSuccess || occ < 1) occ = 1;
-            ab_chunks = (occ * sms) / (B * gx > 0 ? B * gx : 1);
+            ab_chunks = (occ * sms) / (NI * gx > 0 ? NI * gx : 1);
             if (ab_chunks > (L + 7) / 8) ab_chunks = (L + 7) / 8;
             if (ab_chunks < 1) ab_chunks = 1;
         }
         ab_rows = (L + ab_chunks - 1) / ab_chunks;
         ab_chunks = (L + ab_rows - 1) / ab_rows;
     }
+    // attend/fc_1a runs on the NI * L image-level rows: the att_ctx mask of step t is drawn for those rows
     if (side_f) {   // T1[t] = tanh(drop_t(ctx) W1a + b1a) for every step, queued ahead on the second stream
         TCK(hand(st, sd, s->ev[0]));
         for (int t = 0; t < T; ++t) {
-            sat::PackJob job{contexts, nullptr, D, D, BL, 128, s->tc_xpa};
+            sat::PackJob job{contexts, nullptr, D, D, BLi, 128, s->tc_xpa};
             const sat::DropSpec drop{seed, ST(t, 0), kf};
             TCK(sat::pack_rows_launch(&job, 1, lmode, sd, &drop, PDLK));
-            TRET(sat_dense_packed(s->handle, s->tc_xpa, BL, 128, D, s->tc_w1a, s->tc_b1a, A, sat::kEpiBiasTanh, s->T1[t], A, 0, 1, sd));
+            TRET(sat_dense_packed(s->handle, s->tc_xpa, BLi, 128, D, s->tc_w1a, s->tc_b1a, A, sat::kEpiBiasTanh, s->T1[t], A, 0, 1, sd));
             TCK(cudaEventRecord(evT1(t), sd));
         }
     }
+    // the non-fused scorer reads T1 per batch row: grouped, the image blocks of step t are first copied to the rows
+    // (into temp, which att_temp_kernel then updates in place)
+    auto att_t1_rows = [&](int t) -> const float* {
+        if (G == 1) return s->T1[t];
+        launch_k(expand_rows_kernel, GRID1D((size_t)BL * A), 256, st, s->temp, (const float*)s->T1[t], B, L * A, G);
+        return s->temp;
+    };
+    auto launch_ce = [&](int blocks, const float* logits, float* dlogits, int t, int rows_per_step) {
+        if (row_w)
+            launch_k(ce_kernel<true>, blocks, kCeThreads, st, logits, dlogits, sentences, T, t, masks, V, inv_msum, s->loss_acc, rows_per_step, row_w);
+        else
+            launch_k(ce_kernel<false>, blocks, kCeThreads, st, logits, dlogits, sentences, T, t, masks, V, inv_msum, s->loss_acc, rows_per_step,
+                     (const float*)nullptr);
+    };
     // ------------------------------------------------------------ forward through time (model.py:258-312)
     for (int t = 0; t < T; ++t) {
         const float* h_out_prev = t ? s->h_out[t - 1] : s->h0;
         const float* h_state_prev = t ? s->h_state[t - 1] : s->h0;
         const float* c_prev = t ? s->c[t - 1] : s->c0;
         // attend (model.py:395-436)
-        if (!att2) {   // one layer: e = drop(ctx) wa [BL] + drop(h) Wb [B, L]
-            launch_k(dropout2d_kernel, GRID1D((size_t)BL * D), 256, st, s->ctxd, D, contexts, D, BL, D, seed, ST(t, 0), kf, 0);
-            launch_k(rowdot_kernel, (BL * 32 + 255) / 256, 256, st, s->e, s->ctxd, P(vA1aW), BL, D);
+        if (!att2) {   // one layer: e = drop(ctx) wa [BL] + drop(h) Wb [B, L]  (the first term per image)
+            launch_k(dropout2d_kernel, GRID1D((size_t)BLi * D), 256, st, s->ctxd, D, contexts, D, BLi, D, seed, ST(t, 0), kf, 0);
+            launch_k(rowdot_kernel, (BLi * 32 + 255) / 256, 256, st, G > 1 ? s->e_img : s->e, s->ctxd, P(vA1aW), BLi, D);
+            if (G > 1) launch_k(expand_rows_kernel, GRID1D((size_t)BL), 256, st, s->e, (const float*)s->e_img, B, L, G);
         } else if (side_f) {
         } else if (tc) {   // T1 = tanh(drop(ctx) W1a + b1a) on the wgmma dense kernel: the context dropout is applied while the
                     // rows are packed (no fp32 dropped copy), bias + tanh fused in the epilogue
-            sat::PackJob job{contexts, nullptr, D, D, BL, 128, s->tc_xpa};
+            sat::PackJob job{contexts, nullptr, D, D, BLi, 128, s->tc_xpa};
             const sat::DropSpec drop{seed, ST(t, 0), kf};
             TCK(sat::pack_rows_launch(&job, 1, lmode, st, &drop, PDLK));
-            TRET(sat_dense_packed(s->handle, s->tc_xpa, BL, 128, D, s->tc_w1a, s->tc_b1a, A, sat::kEpiBiasTanh, s->T1[t], A, 0, 1, st));
+            TRET(sat_dense_packed(s->handle, s->tc_xpa, BLi, 128, D, s->tc_w1a, s->tc_b1a, A, sat::kEpiBiasTanh, s->T1[t], A, 0, 1, st));
         } else {
-            launch_k(dropout2d_kernel, GRID1D((size_t)BL * D), 256, st, s->ctxd, D, contexts, D, BL, D, seed, ST(t, 0), kf, 0);
-            TRET(dense_fwd(st, s->ctxd, BL, D, P(vA1aW), P(vA1aB), A, s->T1[t], 1));
+            launch_k(dropout2d_kernel, GRID1D((size_t)BLi * D), 256, st, s->ctxd, D, contexts, D, BLi, D, seed, ST(t, 0), kf, 0);
+            TRET(dense_fwd(st, s->ctxd, BLi, D, P(vA1aW), P(vA1aB), A, s->T1[t], 1));
         }
         const bool hd_packed = att2 && pk_fwd_ok(0);
         if (hd_packed)
@@ -1560,20 +1743,20 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
         if (side_f) TCK(cudaStreamWaitEvent(st, evT1(t), 0));
         if (!att2) {   // (the 1-layer scores are complete: e = drop(ctx) wa + drop(h) Wb above)
         } else if (att_fused) {
-            launch_k(att_logits_kernel, (BL * 32 + 255) / 256, 256, st, s->e, s->T1[t], s->q[t], P(vA2W), B, L, A, seed, ST(t, 2), kf);
+            launch_k(att_logits_kernel, (BL * 32 + 255) / 256, 256, st, s->e, s->T1[t], s->q[t], P(vA2W), B, L, A, seed, ST(t, 2), kf, G);
         } else {
-            launch_k(att_temp_kernel, GRID1D((size_t)BL * A), 256, st, s->temp, s->T1[t], s->q[t], B, L, A, seed, ST(t, 2), kf);
+            launch_k(att_temp_kernel, GRID1D((size_t)BL * A), 256, st, s->temp, att_t1_rows(t), s->q[t], B, L, A, seed, ST(t, 2), kf);
             launch_k(rowdot_kernel, (BL * 32 + 255) / 256, 256, st, s->e, s->temp, P(vA2W), BL, A);
         }
         const bool ctx4 = (D & 3) == 0 && (reinterpret_cast<uintptr_t>(contexts) & 15) == 0;
         if (ctx4 && L <= kSmL && fuse_sm) {   // softmax + coverage + context vector in one launch
-            launch_k(softmax_context_fwd4_kernel, dim3((D / 4 + 31) / 32, B), 256, st, s->z[t], s->alpha[t], s->e, contexts, L, D, s->att, masks, T, t);
+            launch_k(softmax_context_fwd4_kernel, dim3((D / 4 + 31) / 32, B), 256, st, s->z[t], s->alpha[t], s->e, contexts, L, D, s->att, masks, T, t, G);
         } else {
             launch_k(softmax_rows_kernel, (B * 32 + 255) / 256, 256, st, s->alpha[t], s->e, B, L, s->att, masks, T, t);   // + coverage
             if (ctx4)   // un-dropped ctx
-                launch_k(context_fwd4_kernel, dim3((D / 4 + 31) / 32, B), 256, st, s->z[t], s->alpha[t], contexts, L, D);
+                launch_k(context_fwd4_kernel, dim3((D / 4 + 31) / 32, B), 256, st, s->z[t], s->alpha[t], contexts, L, D, G);
             else
-                launch_k(context_fwd_kernel, dim3((D + 127) / 128, B), 128, st, s->z[t], s->alpha[t], contexts, B, L, D);
+                launch_k(context_fwd_kernel, dim3((D + 127) / 128, B), 128, st, s->z[t], s->alpha[t], contexts, B, L, D, G);
         }
         // embedding of the previous word: 0 at t = 0, then teacher forcing (model.py:254, 310)
         if (t == 0)   // every step's rows at once (teacher forcing: the words are inputs)
@@ -1602,7 +1785,7 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
             else TRET(dense_fwd(st, s->td[t], B, Dd, P(vD2W), P(vD2B), V, s->logits, 0));
         }
         // masked cross entropy + accuracy, and d loss / d logits (model.py:292-305, 316-318, 332-334)
-        launch_k(ce_kernel, B, kCeThreads, st, s->logits, s->dlogits[t], sentences, T, t, masks, V, inv_msum, s->loss_acc, 0);
+        launch_ce(B, s->logits, s->dlogits[t], t, 0);
     }
     if (dec_all) {   // decode of all T steps (model.py:282-305): the per-step stashes are contiguous = [T*B, .] matrices
         launch_k(concat3_drop_kernel, GRID1D((size_t)TBr * XD), 256, st, s->expd[0], XD, s->h_out[0], H, s->z[0], D, s->emb[0], E, XD, TBr,
@@ -1620,7 +1803,7 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
             TRET(sat_dense_packed(s->handle, s->tc_sx, TBr, s->all_rt, Dd, s->tcl[3].w, s->tcl[3].b, V, sat::kEpiBias, s->logits_all, V, 0,
                                   all_splits(V, Dd), st));
         }
-        launch_k(ce_kernel, TBr, kCeThreads, st, s->logits_all, s->dlogits[0], sentences, T, 0, masks, V, inv_msum, s->loss_acc, B);
+        launch_ce(TBr, s->logits_all, s->dlogits[0], 0, B);
     }
     // attention coverage loss (model.py:320-326) and L2 regulariser (model.py:328)
     launch_k(coverage_loss_kernel, 64, 256, st, s->datt, s->att, BL, s->att_factor, inv_gbl, s->loss_acc);
@@ -1694,27 +1877,39 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
         launch_k(split3_drop_kernel, GRID1D((size_t)B * XL), 256, st, s->dlin, XL, B, s->dz, D, 1, demb, E, 1, s->dh_state, H, 0, D + E, seed,
                                                                    ST(t, 3), kl);
         // attention: context vector, softmax, scorer
-        launch_k(context_bwd_kernel, (BL * 32 + 255) / 256, 256, st, s->dalpha, s->dz, contexts, s->datt, B, L, D, masks, T, t);
+        launch_k(context_bwd_kernel, (BL * 32 + 255) / 256, 256, st, s->dalpha, s->dz, contexts, s->datt, B, L, D, masks, T, t, G);
         const bool sm_in_ab = att2 && att_fused && fuse_env == 1;   // (the fused scorer backward takes the softmax backward itself)
         if (!sm_in_ab) launch_k(softmax_bwd_kernel, (B * 32 + 255) / 256, 256, st, s->dalpha, s->alpha[t], B, L);   // dalpha now holds de
         if (!att2) {   // de = dalpha [B, L]: dwa += drop(ctx)^T de, dWb += drop(h)^T de, d drop(h) = de Wb^T
-            launch_k(dropout2d_kernel, GRID1D((size_t)BL * D), 256, st, s->ctxd, D, contexts, D, BL, D, seed, ST(t, 0), kf, 0);
-            launch_k(colsum_kernel, dim3((D + 127) / 128, (BL + 255) / 256), 128, st, Gd(vA1aW), s->ctxd, BL, D, s->dalpha);
+            launch_k(dropout2d_kernel, GRID1D((size_t)BLi * D), 256, st, s->ctxd, D, contexts, D, BLi, D, seed, ST(t, 0), kf, 0);
+            if (G > 1) launch_k(group_sum_kernel, GRID1D((size_t)BLi), 256, st, s->e_img, (const float*)s->dalpha, NI, L, G);   // de per image
+            launch_k(colsum_kernel, dim3((D + 127) / 128, (BLi + 255) / 256), 128, st, Gd(vA1aW), s->ctxd, BLi, D,
+                     G > 1 ? s->e_img : s->dalpha);
             TRET(dense_bwd(st, s->hd[t], B, H, P(vA1bW), L, s->dalpha, Gd(vA1bW), nullptr, s->dhd));
         } else {
             float* const dtemp = (side_b && (t & 1)) ? s->dtemp2 : s->dtemp;
+            float* dtemp_w = dtemp;   // d temp of the NI * L image-level rows: the fc_1a weight gradient's operand
             if (att_fused) {   // temp, dw2, dtemp, dq, tanh' and (tensor-core path) db1a in one pass over T1
                 if (!stack) TCK(cudaMemsetAsync(dq, 0, (size_t)B * A * sizeof(float), st));   // (stacked: zeroed once before the loop)
                 if (side_b && t + 2 < T) TCK(cudaStreamWaitEvent(st, evRp(t + 2), 0));   // this d temp buffer has been packed
-                launch_k(ab_wave ? att_bwd_fused_wave_kernel : att_bwd_fused_kernel, dim3((A / 4 + kAbCT - 1) / kAbCT, ab_chunks, B),
-                         kAbRG * kAbCT, st, dtemp, dq, Gd(vA2W), tc ? Gd(vA1aB) : nullptr, s->T1[t], s->q[t], s->dalpha, P(vA2W), L, A,
-                         ab_rows, seed, ST(t, 2), kf, sm_in_ab ? s->alpha[t] : nullptr);
+                if (G == 1)
+                    launch_k(ab_wave ? att_bwd_fused_wave_kernel : att_bwd_fused_kernel, dim3((A / 4 + kAbCT - 1) / kAbCT, ab_chunks, B),
+                             kAbRG * kAbCT, st, dtemp, dq, Gd(vA2W), tc ? Gd(vA1aB) : nullptr, s->T1[t], s->q[t], s->dalpha, P(vA2W), L, A,
+                             ab_rows, seed, ST(t, 2), kf, sm_in_ab ? s->alpha[t] : nullptr);
+                else   // one pass over each image's T1 block for all of its rows; d temp summed over the group
+                    launch_k(att_bwd_grouped_kernel, dim3((A / 4 + kAbCT - 1) / kAbCT, ab_chunks, NI), kAbRG * kAbCT, st, dtemp, dq, Gd(vA2W),
+                             tc ? Gd(vA1aB) : nullptr, s->T1[t], s->q[t], s->dalpha, P(vA2W), L, A, ab_rows, G, seed, ST(t, 2), kf,
+                             sm_in_ab ? s->alpha[t] : nullptr);
             } else {
-                launch_k(att_temp_kernel, GRID1D((size_t)BL * A), 256, st, s->temp, s->T1[t], s->q[t], B, L, A, seed, ST(t, 2), kf);
+                launch_k(att_temp_kernel, GRID1D((size_t)BL * A), 256, st, s->temp, att_t1_rows(t), s->q[t], B, L, A, seed, ST(t, 2), kf);
                 launch_k(colsum_kernel, dim3((A + 127) / 128, (BL + 255) / 256), 128, st, Gd(vA2W), s->temp, BL, A, s->dalpha);   // dw2 += temp^T de
                 launch_k(att_dtemp_kernel, GRID1D((size_t)BL * A), 256, st, s->dtemp, s->dalpha, P(vA2W), BL, A, seed, ST(t, 2), kf);
                 launch_k(segsum_kernel, dim3((A + 127) / 128, B), 128, st, dq, s->dtemp, B, L, A);
-                launch_k(tanh_bwd_kernel, GRID1D((size_t)BL * A), 256, st, s->dtemp, s->T1[t], (size_t)BL * A);
+                if (G > 1) {   // sum over each image's rows, then tanh' of the image's T1
+                    launch_k(group_sum_kernel, GRID1D((size_t)BLi * A), 256, st, s->dtemp_g, (const float*)s->dtemp, NI, L * A, G);
+                    dtemp_w = s->dtemp_g;
+                }
+                launch_k(tanh_bwd_kernel, GRID1D((size_t)BLi * A), 256, st, dtemp_w, s->T1[t], (size_t)BLi * A);
             }
             if (tc) {
                 // dW1a[D, A] += ctxd^T[D, BL] * dtemp[BL, A]: the weight repack kernel transposes, so ctxd [BL x D] read
@@ -1722,15 +1917,15 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
                 // packed weight; split-K over an 8-CTA cluster, accumulated into the gradient in the epilogue
                 // (the context dropout mask is re-applied while ctx is packed: mask index row * D + column, as in the forward pass)
                 const sat::DropSpec drop{seed, ST(t, 0), kf};
-                TCK(sat::lin_repack_weight(contexts, BL, D, 0, s->tc_xpa, lmode, sd, &drop, PDLK));   // (needs nothing of this step)
+                TCK(sat::lin_repack_weight(contexts, BLi, D, 0, s->tc_xpa, lmode, sd, &drop, PDLK));   // (needs nothing of this step)
                 if (side_b) TCK(hand(st, sd, evAb(t)));
-                TCK(sat::lin_repack_weight(dtemp, BL, A, 0, s->tc_wbig, lmode, sd, nullptr, PDLK));
+                TCK(sat::lin_repack_weight(dtemp_w, BLi, A, 0, s->tc_wbig, lmode, sd, nullptr, PDLK));
                 if (side_b) TCK(cudaEventRecord(evRp(t), sd));
-                TRET(sat_dense_packed(s->handle, s->tc_xpa, D, 128, BL, s->tc_wbig, nullptr, A, sat::kEpiNone, Gd(vA1aW), A, 1, 8, sd, 1));
-                if (!att_fused) launch_k(colsum_kernel, dim3((A + 127) / 128, (BL + 255) / 256), 128, st, Gd(vA1aB), s->dtemp, BL, A, nullptr);
+                TRET(sat_dense_packed(s->handle, s->tc_xpa, D, 128, BLi, s->tc_wbig, nullptr, A, sat::kEpiNone, Gd(vA1aW), A, 1, 8, sd, 1));
+                if (!att_fused) launch_k(colsum_kernel, dim3((A + 127) / 128, (BLi + 255) / 256), 128, st, Gd(vA1aB), dtemp_w, BLi, A, nullptr);
             } else {
-                launch_k(dropout2d_kernel, GRID1D((size_t)BL * D), 256, st, s->ctxd, D, contexts, D, BL, D, seed, ST(t, 0), kf, 0);
-                TRET(dense_bwd(st, s->ctxd, BL, D, P(vA1aW), A, s->dtemp, Gd(vA1aW), Gd(vA1aB), nullptr));       // contexts are inputs
+                launch_k(dropout2d_kernel, GRID1D((size_t)BLi * D), 256, st, s->ctxd, D, contexts, D, BLi, D, seed, ST(t, 0), kf, 0);
+                TRET(dense_bwd(st, s->ctxd, BLi, D, P(vA1aW), A, dtemp_w, Gd(vA1aW), Gd(vA1aB), nullptr));       // contexts are inputs
             }
             if (pk_dx_ok(0)) {
                 launch_k(tanh_bwd_pack_kernel, GRID1D((size_t)B * A), 256, st, dq, s->q[t], B, A, s->tc_xs, lmode, s->tc_rt);
@@ -1767,17 +1962,25 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
     // ------------------------------------------------------------ initialize backward
     // h0 is both h_out[-1] (attend of step 0) and h_state[-1] (LSTM of step 0); c0 receives dc
     launch_k(copy2d_kernel, GRID1D((size_t)B * H), 256, st, s->dh_out, H, s->dh_state, H, B, H, 1);
-    float* dmid = s->dbuf + (size_t)B * D;  // [B, I]
+    float* dh0 = s->dh_out;
+    float* dc0 = s->dc;
+    if (G > 1) {   // the image's state fed each of its rows: sum their gradients, then initialize backward per image
+        launch_k(group_sum_kernel, GRID1D((size_t)NI * H), 256, st, s->dhi, (const float*)s->dh_out, NI, H, G);
+        launch_k(group_sum_kernel, GRID1D((size_t)NI * H), 256, st, s->dci, (const float*)s->dc, NI, H, G);
+        dh0 = s->dhi;
+        dc0 = s->dci;
+    }
+    float* dmid = s->dbuf + (size_t)B * D;  // [NI, I]
     if (!init2) {
-        TRET(dense_bwd(st, s->meand, B, D, P(vIb1W), H, s->dh_out, Gd(vIb1W), Gd(vIb1B), nullptr));
-        TRET(dense_bwd(st, s->meand, B, D, P(vIa1W), H, s->dc, Gd(vIa1W), Gd(vIa1B), nullptr));
+        TRET(dense_bwd(st, s->meand, NI, D, P(vIb1W), H, dh0, Gd(vIb1W), Gd(vIb1B), nullptr));
+        TRET(dense_bwd(st, s->meand, NI, D, P(vIa1W), H, dc0, Gd(vIa1W), Gd(vIa1B), nullptr));
     } else {
-        TRET(dense_bwd(st, s->ib1d, B, I, P(vIb2W), H, s->dh_out, Gd(vIb2W), Gd(vIb2B), dmid));
-        launch_k(drop_tanh_bwd_kernel, GRID1D((size_t)B * I), 256, st, dmid, s->ib1, (size_t)B * I, seed, INIT + 2, kf, (size_t)0);
-        TRET(dense_bwd(st, s->meand, B, D, P(vIb1W), I, dmid, Gd(vIb1W), Gd(vIb1B), nullptr));
-        TRET(dense_bwd(st, s->ia1d, B, I, P(vIa2W), H, s->dc, Gd(vIa2W), Gd(vIa2B), dmid));
-        launch_k(drop_tanh_bwd_kernel, GRID1D((size_t)B * I), 256, st, dmid, s->ia1, (size_t)B * I, seed, INIT + 1, kf, (size_t)0);
-        TRET(dense_bwd(st, s->meand, B, D, P(vIa1W), I, dmid, Gd(vIa1W), Gd(vIa1B), nullptr));
+        TRET(dense_bwd(st, s->ib1d, NI, I, P(vIb2W), H, dh0, Gd(vIb2W), Gd(vIb2B), dmid));
+        launch_k(drop_tanh_bwd_kernel, GRID1D((size_t)NI * I), 256, st, dmid, s->ib1, (size_t)NI * I, seed, INIT + 2, kf, (size_t)0);
+        TRET(dense_bwd(st, s->meand, NI, D, P(vIb1W), I, dmid, Gd(vIb1W), Gd(vIb1B), nullptr));
+        TRET(dense_bwd(st, s->ia1d, NI, I, P(vIa2W), H, dc0, Gd(vIa2W), Gd(vIa2B), dmid));
+        launch_k(drop_tanh_bwd_kernel, GRID1D((size_t)NI * I), 256, st, dmid, s->ia1, (size_t)NI * I, seed, INIT + 1, kf, (size_t)0);
+        TRET(dense_bwd(st, s->meand, NI, D, P(vIa1W), I, dmid, Gd(vIa1W), Gd(vIa1B), nullptr));
     }
     TCK(cudaGetLastError());
     TCK(cudaMemcpyAsync(losses, s->loss_acc, 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -1786,16 +1989,50 @@ static int train_enqueue(TrainState* s, const float* params, float* grads, const
 
 namespace {
 __global__ void reciprocal_kernel(float* out, const double* in) { *out = (float)(1.0 / *in); }
+
+// masks[r, t] = 1 up to and including the first eos of row r (every t if there is none), 0 after it; *sum = their total
+// (one CTA: a deterministic sum, and the rows x T of a sampling round are few)
+__global__ void __launch_bounds__(256) caption_masks_kernel(const int32_t* __restrict__ tokens, int rows, int T, int eos,
+                                                            float* __restrict__ masks, double* sum) {
+    __shared__ double red[8];
+    double s = 0.0;
+    for (int r = threadIdx.x; r < rows; r += blockDim.x) {
+        const int32_t* tk = tokens + (size_t)r * T;
+        int end = T;   // number of words kept
+        for (int t = 0; t < T; ++t)
+            if (tk[t] == eos) { end = t + 1; break; }
+        float* m = masks + (size_t)r * T;
+        for (int t = 0; t < T; ++t) m[t] = t < end ? 1.f : 0.f;
+        s += end;
+    }
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0 && sum) {
+        double tot = 0.0;
+        for (int w = 0; w < (int)blockDim.x / 32; ++w) tot += red[w];
+        *sum = tot;
+    }
+}
 }  // namespace
 
+extern "C" int sat_caption_masks(const int32_t* tokens, int32_t rows, int32_t T, int32_t eos_id, float* masks, double* mask_sum,
+                                 void* stream) {
+    if (!tokens || !masks || rows < 0 || T < 1) return sat_fail(SAT_ERR_INVALID, "sat_caption_masks: bad argument");
+    caption_masks_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(tokens, rows, T, eos_id, masks, mask_sum);
+    TCK(cudaGetLastError());
+    return SAT_OK;
+}
+
 static int train_forward_backward(sat_handle* h, const float* params, float* grads, const float* contexts,
-                                  const int32_t* sentences, const float* masks, int32_t B, int32_t T, uint64_t seed,
-                                  double global_mask_sum, const double* global_mask_sum_dev, int32_t global_batch, float* losses,
-                                  void* stream) {
+                                  const int32_t* sentences, const float* masks, const float* row_w, int32_t n_img,
+                                  int32_t group, int32_t T, uint64_t seed, double global_mask_sum, const double* global_mask_sum_dev,
+                                  int32_t global_batch, float* losses, void* stream) {
     if (!h || !params || !grads || !contexts || !sentences || !masks || !losses)
         return sat_fail(SAT_ERR_INVALID, "sat_train_forward_backward: null argument");
     TrainState* s = (TrainState*)*sat_handle_train_slot(h);
-    if (!s || s->B != B || s->T != T) return sat_fail(SAT_ERR_STATE, "call sat_train_init(B=%d, T=%d) first", B, T);
+    const int32_t B = n_img * group;
+    if (!s || s->n_img * s->group != B || s->T != T) return sat_fail(SAT_ERR_STATE, "call sat_train_init(B=%d, T=%d) first", B, T);
     TCK(cudaSetDevice(sat_handle_device(h)));
     cudaStream_t st = (cudaStream_t)stream;
     // per-call scalars -> device cells, in stream order.  The sources are ordinary (pageable) host variables: such a
@@ -1806,11 +2043,12 @@ static int train_forward_backward(sat_handle* h, const float* params, float* gra
     TCK(cudaMemcpyAsync(s->seed_d, &seed_v, 8, cudaMemcpyHostToDevice, st));
     if (global_mask_sum_dev) reciprocal_kernel<<<1, 1, 0, st>>>(s->inv_msum_d, global_mask_sum_dev);   // the sum never visits the host
     else TCK(cudaMemcpyAsync(s->inv_msum_d, &inv, 4, cudaMemcpyHostToDevice, st));
-    auto enqueue = [&]() { return train_enqueue(s, params, grads, contexts, sentences, masks, B, T, global_batch, losses, st); };
+    auto enqueue = [&]() { return train_enqueue(s, params, grads, contexts, sentences, masks, row_w, B, T, global_batch, losses, st); };
     if (st == nullptr || st == cudaStreamLegacy || st == cudaStreamPerThread) return enqueue();
+    // (row weights are read on the device: new values in the same buffer replay the graph)
     std::vector<long long> key = {(long long)params, (long long)grads, (long long)contexts, (long long)sentences,
                                   (long long)masks, (long long)losses, B, T, global_batch,
-                                  sat_handle_train_tc(h), sat_handle_layout_mode(h)};
+                                  sat_handle_train_tc(h), sat_handle_layout_mode(h), group, (long long)row_w};
     TrainState::GEntry* ent = nullptr;
     for (auto& g : s->graphs)
         if (g.key == key) ent = &g;
@@ -1842,8 +2080,11 @@ extern "C" int sat_train_forward_backward(sat_handle* h, const float* params, fl
                                           const int32_t* sentences, const float* masks, int32_t B, int32_t T,
                                           uint64_t seed, double global_mask_sum, int32_t global_batch, float* losses,
                                           void* stream) {
-    return train_forward_backward(h, params, grads, contexts, sentences, masks, B, T, seed, global_mask_sum, nullptr, global_batch,
-                                  losses, stream);
+    TrainState* s = h ? (TrainState*)*sat_handle_train_slot(h) : nullptr;
+    if (s && s->group != 1 && s->B == B && s->T == T)
+        return sat_fail(SAT_ERR_STATE, "the training state is grouped (%d x %d): use sat_train_forward_backward_grouped", s->n_img, s->group);
+    return train_forward_backward(h, params, grads, contexts, sentences, masks, nullptr, B, 1, T, seed, global_mask_sum, nullptr,
+                                  global_batch, losses, stream);
 }
 // the same with the global mask sum in device memory (one double, e.g. the result of an all-reduce still in flight
 // on `stream`): a data-parallel loop then has no host synchronisation per step
@@ -1852,8 +2093,28 @@ extern "C" int sat_train_forward_backward_dsum(sat_handle* h, const float* param
                                                uint64_t seed, const double* global_mask_sum_dev, int32_t global_batch,
                                                float* losses, void* stream) {
     if (!global_mask_sum_dev) return sat_fail(SAT_ERR_INVALID, "sat_train_forward_backward_dsum: null mask sum");
-    return train_forward_backward(h, params, grads, contexts, sentences, masks, B, T, seed, 1.0, global_mask_sum_dev, global_batch,
-                                  losses, stream);
+    TrainState* s = h ? (TrainState*)*sat_handle_train_slot(h) : nullptr;
+    if (s && s->group != 1 && s->B == B && s->T == T)
+        return sat_fail(SAT_ERR_STATE, "the training state is grouped (%d x %d): use sat_train_forward_backward_grouped", s->n_img, s->group);
+    return train_forward_backward(h, params, grads, contexts, sentences, masks, nullptr, B, 1, T, seed, 1.0, global_mask_sum_dev,
+                                  global_batch, losses, stream);
+}
+// rows = n_img * group captions, row r of image r / group; contexts [n_img, L, D]; row_w [rows] or NULL (= 1)
+extern "C" int sat_train_forward_backward_grouped(sat_handle* h, const float* params, float* grads, const float* contexts,
+                                                  int32_t n_img, int32_t group, const int32_t* sentences, const float* masks,
+                                                  const float* row_weights, int32_t T, uint64_t seed,
+                                                  const double* global_mask_sum_dev, int32_t global_batch, float* losses,
+                                                  void* stream) {
+    if (!h || !params || !grads || !contexts || !sentences || !masks || !losses || !global_mask_sum_dev)
+        return sat_fail(SAT_ERR_INVALID, "sat_train_forward_backward_grouped: null argument");
+    if (group < 1 || n_img < 1 || T < 1) return sat_fail(SAT_ERR_INVALID, "sat_train_forward_backward_grouped: bad n_img/group/T");
+    TrainState* s = (TrainState*)*sat_handle_train_slot(h);
+    if (!s) return sat_fail(SAT_ERR_STATE, "call sat_train_init_grouped first");
+    if (s->n_img != n_img || s->group != group || s->T != T)
+        return sat_fail(SAT_ERR_INVALID, "sat_train_forward_backward_grouped: (n_img, group, T) = (%d, %d, %d), the state has (%d, %d, %d)",
+                        n_img, group, T, s->n_img, s->group, s->T);
+    return train_forward_backward(h, params, grads, contexts, sentences, masks, row_weights, n_img, group, T, seed, 1.0,
+                                  global_mask_sum_dev, global_batch, losses, stream);
 }
 
 // grads: the (all-reduced) sum over data-parallel shards.  Adds the L2-regulariser gradient once, clips by the

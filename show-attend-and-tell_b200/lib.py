@@ -69,6 +69,9 @@ SIGNATURES = {
                                 C.POINTER(_I), C.POINTER(_L)]),
     "sat_train_forward_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _I, C.c_uint64, C.c_double, _I, _P, _P]),
     "sat_train_forward_backward_dsum": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _I, C.c_uint64, _P, _I, _P, _P]),
+    "sat_train_init_grouped": (C.c_int, [_P, _I, _I, _I, C.c_float, C.c_float, C.c_float, C.c_float]),
+    "sat_train_forward_backward_grouped": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _I, C.c_uint64, _P, _I, _P, _P]),
+    "sat_caption_masks": (C.c_int, [_P, _I, _I, _I, _P, _P, _P]),
     "sat_train_apply": (C.c_int, [_P, _P, _P, _P, _P, _L, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, _P,
                                   _P]),
     "sat_train_apply_opt": (C.c_int, [_P, _P, _P, _P, _P, _P, _L, C.POINTER(Optimizer), _P, _P]),

@@ -162,8 +162,9 @@ class CaptionGenerator(object):
     def variable_names(self):
         return list(self._shapes)
 
-    def set_weights(self, weights):
-        """weights: {tf_variable_name[:0]: ndarray/tensor} in the reference layouts."""
+    def set_weights(self, weights, sync=True):
+        """weights: {tf_variable_name[:0]: ndarray/tensor} in the reference layouts.  sync=False skips the final host
+        synchronisation: only for CUDA tensors that outlive the queued repack (e.g. views of the training parameters)."""
         torch = self.torch
         given = {(k[:-2] if k.endswith(":0") else k): v for k, v in weights.items()}
         keep = []
@@ -181,7 +182,7 @@ class CaptionGenerator(object):
             self._sync_in()                     # (the upload / cast above ran on the caller's stream: a stream wait, no host sync)
             self._check(self.lib.sat_set_weight(self._h, name.encode(), self._p(w), rows, cols, self._st()))
             keep.append(w)                      # the repack is asynchronous: the source lives until the stream is past it
-        if keep:
+        if keep and sync:
             self.stream.synchronize()           # ONE synchronisation per call (it was one per variable)
         return self.lib.sat_weights_missing(self._h)
 
@@ -192,18 +193,27 @@ class CaptionGenerator(object):
         return len(self._shapes) - missing
 
     # ------------------------------------------------------------------ training step (base_model.py:39-68)
-    def train_setup(self, batch_size, num_steps=None, weights=None):
+    def train_setup(self, batch_size, num_steps=None, weights=None, group=1):
         """Allocate the flat parameter / gradient / Adam buffers for training with `batch_size` images per
         process and `num_steps` unrolled time steps (config.max_caption_length).  `weights`: initial values
         (dict of TF variable names); default U(-s, s) kernels and zero biases like the reference
-        (utils/nn.py:29-31).  The reference's trainable set (model.py:225: embedding, dense layers, LSTM)."""
+        (utils/nn.py:29-31).  The reference's trainable set (model.py:225: embedding, dense layers, LSTM).
+        group > 1: `group` captions per image (batch_size * group rows, row r of image r // group) with the image's
+        contexts shared by its rows (sat_train_init_grouped): train_forward_backward(..., group=group), scst_step."""
         torch = self.torch
         cfg = self.config
         T = int(num_steps or cfg.max_caption_length)
-        self._check(self.lib.sat_train_init(self._h, int(batch_size), T, float(cfg.fc_drop_rate),
-                                            float(cfg.lstm_drop_rate), float(cfg.attention_loss_factor),
-                                            float(cfg.fc_kernel_regularizer_scale)))
-        self._train_BT = (int(batch_size), T)
+        group = int(group)
+        if group == 1:
+            self._check(self.lib.sat_train_init(self._h, int(batch_size), T, float(cfg.fc_drop_rate),
+                                                float(cfg.lstm_drop_rate), float(cfg.attention_loss_factor),
+                                                float(cfg.fc_kernel_regularizer_scale)))
+        else:
+            self._check(self.lib.sat_train_init_grouped(self._h, int(batch_size), group, T, float(cfg.fc_drop_rate),
+                                                        float(cfg.lstm_drop_rate), float(cfg.attention_loss_factor),
+                                                        float(cfg.fc_kernel_regularizer_scale)))
+        self._train_BT = (int(batch_size) * group, T)
+        self._train_group = (int(batch_size), group)
         n = self.lib.sat_train_num_vars(self._h)
         self._train_vars = []
         total = C.c_int64()
@@ -261,16 +271,28 @@ class CaptionGenerator(object):
         buf = dict(params=self.params, grads=self.grads, m=self.adam_m, v=self.adam_v)[which]
         return {nm: self._var_view(buf, nm) for nm, *_ in self._train_vars}
 
-    def sync_inference_weights(self):
-        """Repack the trained parameters for the decode kernels (so beam_search / decode_step use them)."""
-        return self.set_weights(self.train_state_dict("params"))
+    def sync_inference_weights(self, sync=True):
+        """Repack the trained parameters for the decode kernels (so beam_search / decode_step use them).  sync=False:
+        no host synchronisation (the sources are views of the persistent self.params, which outlive the queued repack);
+        the decode calls that follow on the same stream see the new weights."""
+        return self.set_weights(self.train_state_dict("params"), sync=sync)
 
-    def train_forward_backward(self, contexts, sentences, masks, seed=None, global_mask_sum=None, global_batch=None):
+    def train_forward_backward(self, contexts, sentences, masks, seed=None, global_mask_sum=None, global_batch=None,
+                               group=1, row_weights=None):
         """Forward + backward of one batch shard; fills self.grads (no regulariser term) and returns the device
-        tensor of the four losses (cross_entropy, accuracy, attention, reg).  seed: see _step_seed."""
+        tensor of the four losses (cross_entropy, accuracy, attention, reg).  seed: see _step_seed.
+        group > 1 (the group of train_setup): contexts [n_img, L, D] are shared by the `group` caption rows of each
+        image (sentences / masks [n_img * group, T]).  row_weights [rows] (or None = 1) multiply each row's cross entropy
+        and its gradient (sat_train_forward_backward_grouped)."""
         seed = self._step_seed(seed)
         torch = self.torch
         B, T = self._train_BT
+        n_img, G = getattr(self, "_train_group", (B, 1))
+        if int(group) != G:
+            raise ValueError("group=%d, but train_setup was called with group=%d" % (int(group), G))
+        if G > 1 or row_weights is not None:
+            return self._train_forward_backward_grouped(contexts, sentences, masks, seed, global_mask_sum, global_batch,
+                                                        row_weights)
         ctx = self._dev(contexts, torch.float32)
         sent = self._dev(sentences, torch.int32)
         mk = self._dev(masks, torch.float32)
@@ -293,6 +315,35 @@ class CaptionGenerator(object):
                                                         self._p(self._train_losses), self._st()))
         self._sync_out()
         self._keep["train_in"] = (ctx, sent, mk)
+        return self._train_losses
+
+    def _train_forward_backward_grouped(self, contexts, sentences, masks, seed, global_mask_sum, global_batch, row_weights):
+        torch = self.torch
+        B, T = self._train_BT
+        n_img, G = self._train_group
+        ctx = self._dev(contexts, torch.float32)
+        sent = self._dev(sentences, torch.int32)
+        mk = self._dev(masks, torch.float32)
+        if tuple(sent.shape) != (B, T) or tuple(mk.shape) != (B, T) or ctx.shape[0] != n_img:
+            raise ValueError("grouped step: contexts [%d, L, D] and sentences / masks [%d, %d] expected, got %s, %s, %s"
+                             % (n_img, B, T, tuple(ctx.shape), tuple(sent.shape), tuple(mk.shape)))
+        w = None if row_weights is None else self._dev(row_weights, torch.float32).reshape(-1)
+        if w is not None and w.numel() != B:
+            raise ValueError("row_weights: %d values for %d rows" % (w.numel(), B))
+        gb = B if global_batch is None else int(global_batch)
+        if isinstance(global_mask_sum, torch.Tensor):
+            gsum = global_mask_sum
+            assert gsum.is_cuda and gsum.dtype == torch.float64 and gsum.numel() == 1
+        else:   # (the grouped entry reads the sum from device memory)
+            v = self._mask_sum(masks, mk) if global_mask_sum is None else float(global_mask_sum)
+            gsum = self._buf("train_msum", (1,), torch.float64)
+            gsum.fill_(v)
+        self._sync_in()
+        self._check(self.lib.sat_train_forward_backward_grouped(self._h, self._p(self.params), self._p(self.grads), self._p(ctx),
+                                                                n_img, G, self._p(sent), self._p(mk), self._p(w), T, int(seed),
+                                                                self._p(gsum), gb, self._p(self._train_losses), self._st()))
+        self._sync_out()
+        self._keep["train_in"] = (ctx, sent, mk, w, gsum)
         return self._train_losses
 
     def _mask_sum(self, masks, mk):
@@ -404,20 +455,12 @@ class CaptionGenerator(object):
         import torch.distributed as dist
         dist.all_reduce(self._flat)
 
-    def train_step(self, contexts, sentences, masks, seed=None, sync=True, next_masks=None):
-        """One optimisation step (the sess.run(opt_op) of base_model.py:57-60) on this process's shard; with
-        torch.distributed initialised the gradients are summed over the ranks by ONE all-reduce of the flat
-        buffer (NCCL) and the losses are normalised by the global batch.  sync=False returns the device tensors
-        (losses [4], squared gradient norm [1]) without reading them back, so that the host can queue the next step
-        while this one runs (the reference reads its summary every step; a training loop rarely needs to).
-        seed: see _step_seed (None = new dropout masks every step, 0 = dropout off).
-        next_masks (data parallel): the masks the NEXT call will be given, if the input pipeline already has them: their
-        sum then rides in this step's gradient collective and the next step starts without a collective of its own
-        (a promise — only the shape is checked; default: the same masks tensor is expected again)."""
+    def _shard_forward_backward(self, mk, seed, next_masks, fb):
+        """The data-parallel protocol of one step around fb(seed, global_mask_sum, global_batch) -> losses [4] (device).
+        Single process: fb gets the step's seed, None (the local mask sum) and the row count."""
         import torch.distributed as dist
         torch = self.torch
         B, T = self._train_BT
-        mk = self._dev(masks, torch.float32)
         world = dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1
         if world > 1:
             # ONE collective per step: the flat buffer [gradients | ce, accuracy, attention sums | mask sum of the NEXT
@@ -429,12 +472,98 @@ class CaptionGenerator(object):
             gsum = self._dp.global_mask_sum(mk)
             seed = self._step_seed(seed)
             seed = seed + 0x1000003 * dist.get_rank() if seed else 0   # rank-offset mask streams (0 stays "off")
-            losses = self.train_forward_backward(contexts, sentences, mk, seed, gsum, B * world)
-            losses = torch.cat([self._dp.reduce(losses, nxt, announced=next_masks is not None), losses[3:4]])   # the single collective of the step
-        else:
-            seed = self._step_seed(seed)
-            msum = self._mask_sum(masks, mk)
-            losses = self.train_forward_backward(contexts, sentences, mk, seed, msum, B * world)
+            losses = fb(seed, gsum, B * world)
+            return torch.cat([self._dp.reduce(losses, nxt, announced=next_masks is not None), losses[3:4]])   # the single collective of the step
+        return fb(self._step_seed(seed), None, B)
+
+    def scst_step(self, contexts, reward_fn, num_samples=5, baseline="greedy", temperature=1.0, seed=None,
+                  sample_seed=None, sync=True):
+        """One self-critical (SCST) policy-gradient step on a shard of images.
+
+          1. the decode weights are refreshed from the training parameters (no host synchronisation);
+          2. num_samples = K captions per image are drawn (sample_device, sample_seed);
+          3. baseline "greedy": the greedy caption of each image is decoded as well;
+          4. reward_fn(captions) is called once: captions[i] is the list of image i's word-id lists, each cut after its
+             first eos_id: the K samples, then the greedy caption for baseline "greedy".  It returns rewards [n, K + 1]
+             ("greedy") or [n, K] ("mean");
+          5. advantages = sample reward - baseline: the greedy caption's reward, or for "mean" the mean reward of the
+             image's other K - 1 samples (captions.scst_advantages);
+          6. the caption masks and their sum are built on the device (sat_caption_masks);
+          7. the grouped step with the advantages as row weights minimises sum_r A_r sum_t m_rt (-log p(w_rt)) / sum m
+             (plus the attention loss), with the image's contexts shared by its K rows; seed: the training dropout
+             (see _step_seed; 0 = off, which makes the step exactly on-policy: sampling runs without dropout);
+          8. train_apply (clip + optimizer).
+        Needs train_setup(n_img, group=num_samples).  With torch.distributed initialised, the mask sum of the whole
+        batch and the gradient sum travel in train_step's single collective.  Returns the losses, the mean sample
+        reward, the mean baseline reward and the gradient norm (sync=False: the losses [4] and the squared gradient
+        norm [1] as device tensors, the rewards as floats)."""
+        from .captions import cut_after_eos, scst_advantages
+        torch = self.torch
+        cfg = self.config
+        K = int(num_samples)
+        if baseline not in ("greedy", "mean"):
+            raise ValueError("baseline must be 'greedy' or 'mean', got %r" % (baseline,))
+        if K < 1 or (baseline == "mean" and K < 2):
+            raise ValueError("num_samples=%d: at least 1 (baseline 'greedy') or 2 (baseline 'mean')" % K)
+        ctx = self._dev(contexts, torch.float32)
+        n = int(ctx.shape[0])
+        if getattr(self, "_train_group", None) != (n, K):
+            raise ValueError("scst_step on %d images x %d samples needs train_setup(%d, group=%d)" % (n, K, n, K))
+        rows = n * min(K, self.SAMPLE_GROUP)
+        if rows > self.max_batch:
+            raise ValueError("sampling %d images x %d captions per call needs max_batch >= %d (the handle has %d)"
+                             % (n, min(K, self.SAMPLE_GROUP), rows, self.max_batch))
+        B, T = self._train_BT
+        eos = int(cfg.eos_id)
+        self.sync_inference_weights(sync=False)
+        tokens, _ = self.sample_device(ctx, K, T, temperature, sample_seed, want_word_probs=False)
+        sent = self._buf("scst_sent", (B, T), torch.int32)
+        with torch.cuda.stream(self.stream):
+            sent.copy_(tokens.reshape(B, T))
+        greedy = self.loop_device(ctx, T)[0] if baseline == "greedy" else None
+        self.stream.synchronize()
+        toks = sent.cpu().numpy().reshape(n, K, T)
+        gt = greedy.cpu().numpy() if greedy is not None else None
+        caps = [[cut_after_eos(toks[i, k], eos) for k in range(K)] + ([cut_after_eos(gt[i], eos)] if gt is not None else [])
+                for i in range(n)]
+        adv, r_sample, r_base = scst_advantages(reward_fn(caps), K, baseline)
+        w = self._buf("scst_w", (B,), torch.float32)
+        w.copy_(torch.from_numpy(np.ascontiguousarray(adv.reshape(-1), dtype=np.float32)))
+        mk = self._buf("scst_masks", (B, T), torch.float32)
+        msum = self._buf("scst_msum", (1,), torch.float64)
+        self._sync_in()
+        self._check(self.lib.sat_caption_masks(self._p(sent), B, T, eos, self._p(mk), self._p(msum), self._st()))
+        self._sync_out()
+        torch.autograd.graph.increment_version(mk)   # (written in place by the library: new masks for StepCollective)
+        losses = self._shard_forward_backward(
+            mk, seed, None,
+            lambda sd, gsum, gb: self.train_forward_backward(ctx, sent, mk, sd, msum if gsum is None else gsum, gb,
+                                                             group=K, row_weights=w))
+        norm2 = self.train_apply()
+        if not sync:
+            return dict(losses=losses, gradient_norm2=norm2, sample_reward=r_sample, baseline_reward=r_base)
+        ce, acc, att, reg = [float(x) for x in losses.tolist()]
+        return dict(cross_entropy_loss=ce, accuracy=acc, attention_loss=att, reg_loss=reg, total_loss=ce + att + reg,
+                    sample_reward=r_sample, baseline_reward=r_base, gradient_norm=float(norm2.item()) ** 0.5,
+                    global_step=self.global_step)
+
+    def train_step(self, contexts, sentences, masks, seed=None, sync=True, next_masks=None):
+        """One optimisation step (the sess.run(opt_op) of base_model.py:57-60) on this process's shard; with
+        torch.distributed initialised the gradients are summed over the ranks by ONE all-reduce of the flat
+        buffer (NCCL) and the losses are normalised by the global batch.  sync=False returns the device tensors
+        (losses [4], squared gradient norm [1]) without reading them back, so that the host can queue the next step
+        while this one runs (the reference reads its summary every step; a training loop rarely needs to).
+        seed: see _step_seed (None = new dropout masks every step, 0 = dropout off).
+        next_masks (data parallel): the masks the NEXT call will be given, if the input pipeline already has them: their
+        sum then rides in this step's gradient collective and the next step starts without a collective of its own
+        (a promise — only the shape is checked; default: the same masks tensor is expected again)."""
+        torch = self.torch
+        mk = self._dev(masks, torch.float32)
+        losses = self._shard_forward_backward(
+            mk, seed, next_masks,
+            lambda sd, gsum, gb: self.train_forward_backward(contexts, sentences, mk, sd,
+                                                             self._mask_sum(masks, mk) if gsum is None else gsum, gb,
+                                                             group=self._train_group[1]))
         norm2 = self.train_apply()
         if not sync:
             return losses, norm2
