@@ -179,6 +179,22 @@ int sat_beam_search_maps(sat_handle* h, const float* contexts, int32_t n_img, in
  * CaptionGenerator.sample does). */
 int sat_sample_loop(sat_handle* h, const float* contexts, int32_t n_img, int32_t num_samples, int32_t T,
                     float temperature, uint64_t seed, int32_t* tokens, float* word_probs, void* stream);
+/* sat_sample_loop_filtered: sat_sample_loop with the two filters of text generation, applied after the temperature.
+ * Words of a row rank by (logit desc, index asc).  top_k >= 1 keeps the first top_k words of that order (0, or
+ * top_k >= V: all words); top_p in (0, 1) then keeps the shortest prefix, in the same order, of those words whose
+ * softmax(logits / temperature), renormalised over them, sums to top_p or more (1: all of them).  At least one word is
+ * always kept.  The draw is sat_sample_loop's Gumbel arg-max restricted to the kept words: when the unfiltered draw of
+ * the same (seed, r, t) is kept, it is the filtered draw too.  word_probs keep sat_sample_loop's meaning (the model's
+ * probability of the word at temperature 1 over the whole vocabulary, not a filtered probability).
+ * With a filter on, the vocabulary layer writes the logits and a per-row kernel selects the kept words (integer radix
+ * selection; the nucleus mass is summed in 64-bit fixed point, so the result does not depend on the launch) and
+ * draws; top_k == 0 && top_p == 1 runs exactly sat_sample_loop.  top_k and top_p, like seed and temperature, are not
+ * part of the CUDA-graph key: new values replay the captured graph.
+ * Errors: those of sat_sample_loop, and SAT_ERR_INVALID for top_k < 0 or top_p NaN, <= 0 or > 1 (nothing is
+ * enqueued). */
+int sat_sample_loop_filtered(sat_handle* h, const float* contexts, int32_t n_img, int32_t num_samples, int32_t T,
+                             float temperature, int32_t top_k, float top_p, uint64_t seed, int32_t* tokens,
+                             float* word_probs, void* stream);
 /* the uniform variate behind the Gumbel noise of (seed, row, step, word), u = (bits + 0.5) * 2^-32 in (0, 1), computed
  * on the host (tests rebuild every draw with it) */
 double sat_sample_uniform(uint64_t seed, int64_t row, int32_t step, int32_t word);

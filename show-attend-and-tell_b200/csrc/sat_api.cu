@@ -1148,7 +1148,8 @@ static int step_impl(sat_handle* h, StepIO& io, cudaStream_t st) {
     RET(attention_impl(h, io.ctx, io.n_img, io.group, io.h_in, io.alpha, h->z, st, io.q_ready, io.last_word));
     RET(lstm_impl(h, h->z, io.last_word, io.c_in, io.h_in, io.c_out, io.h_out, rows, st));
     float* logits = io.logits ? io.logits : h->logits;
-    const bool argmax_only = io.want_rows && !io.probs && io.rows.topk == 0 && !io.rows.argmax;
+    // (a filtered draw needs the row's logits: the per-row kernel makes it after the vocabulary layer)
+    const bool argmax_only = io.want_rows && !io.probs && io.rows.topk == 0 && !io.rows.argmax && !io.rows.filter;
     int fused = 0;
     RET(decode_impl(h, io.h_out, h->z, io.last_word, logits, rows, st, io.make_next_q,
                     argmax_only ? &io.rows : nullptr, &fused));
@@ -1157,6 +1158,10 @@ static int step_impl(sat_handle* h, StepIO& io, cudaStream_t st) {
         rp.logits = logits;
         rp.V = h->d.vocabulary_size;
         rp.probs = io.probs;
+        if (rp.filter && h->opt_trace == 3 && h->tl_count < 4000) {
+            rp.tl = h->trace + 4 * h->tl_count++;
+            h->tl_names.push_back("filter/" + std::to_string(rows));
+        }
         {
             ProfScope ps(h, kTagRows, st);
             CK(rows_softmax_launch(rp, rows, st));
@@ -1550,11 +1555,13 @@ static bool vocab_argmax_fits(sat_handle* h, int B) {
 }
 
 // G, smp: see loop_enqueue_overlap (the sampling loop runs G = num_samples rows per image)
+// filter: filtered sampling (smp->top_k / top_p): the per-step layout, the vocabulary layer writes the logits and the
+// filtered per-row kernel draws (the overlapped and chained layouts need the fused arg-max)
 static int loop_enqueue(sat_handle* h, const float* ctx, int B, int T, const int32_t* forced, int32_t* tokens,
                         float* logits_all, float* alphas, float* word_probs, cudaStream_t st, int G = 1,
-                        const SampleParams* smp = nullptr) {
+                        const SampleParams* smp = nullptr, bool filter = false) {
     const bool pa = h->pa_ok && h->opt_pa && h->opt_gemm != 0;
-    const bool am = pa && vocab_argmax_fits(h, B);
+    const bool am = pa && vocab_argmax_fits(h, B) && !filter;
     const bool maps = alphas || word_probs;   // (the experimental chained launch takes no maps, and does not sample)
     if (!maps && !smp && fused_loop_available(h, B)) return loop_enqueue_fused(h, ctx, B, T, forced, tokens, logits_all, st, false);
     if (am && h->opt_overlap == 2 && h->opt_pdl && h->d.num_decode_layers == 2)
@@ -1577,6 +1584,7 @@ static int loop_enqueue(sat_handle* h, const float* ctx, int B, int T, const int
         io.rows.next_word = h->word; io.rows.forced = forced; io.rows.forced_ld = T;
         io.rows.word_probs = word_probs;
         io.rows.sample = smp;
+        io.rows.filter = filter ? 1 : 0;
         io.q_ready = t > 0;
         io.make_next_q = t + 1 < T;
         io.pa_slot = t & 1;          // initialize / the previous LSTM wrote the packed h into this slot
@@ -1715,6 +1723,40 @@ extern "C" int sat_sample_loop(sat_handle* h, const float* contexts, int32_t n_i
     std::vector<long long> key = {5, (long long)contexts, n_img, num_samples, T, (long long)tokens, (long long)word_probs};
     const int rc = run_graphed(h, key, st, [&]() -> int {
         return loop_enqueue(h, contexts, B, T, nullptr, tokens, nullptr, nullptr, word_probs, st, num_samples, h->smp);
+    });
+    note_projected(h, rc == SAT_OK ? contexts : nullptr, n_img);   // (see sat_decode_loop)
+    return rc;
+}
+
+extern "C" int sat_sample_loop_filtered(sat_handle* h, const float* contexts, int32_t n_img, int32_t num_samples,
+                                        int32_t T, float temperature, int32_t top_k, float top_p, uint64_t seed,
+                                        int32_t* tokens, float* word_probs, void* stream) {
+    if (!h) return fail(SAT_ERR_INVALID, "null handle");
+    if (top_k < 0) return fail(SAT_ERR_INVALID, "top_k %d < 0", top_k);
+    if (!(top_p > 0.0f && top_p <= 1.0f)) return fail(SAT_ERR_INVALID, "top_p %g outside (0, 1]", (double)top_p);
+    if (top_k == 0 && top_p == 1.0f)
+        return sat_sample_loop(h, contexts, n_img, num_samples, T, temperature, seed, tokens, word_probs, stream);
+    if (!contexts || !tokens) return fail(SAT_ERR_INVALID, "sat_sample_loop_filtered: null tensor");
+    if (!(temperature > 0.0f) || !isfinite(temperature) || !isfinite(1.0f / temperature))
+        return fail(SAT_ERR_INVALID, "temperature %g must be positive and finite", (double)temperature);
+    if (num_samples < 1) return fail(SAT_ERR_INVALID, "num_samples %d < 1", num_samples);
+    if (n_img < 1 || (long long)n_img * num_samples > h->max_rows)
+        return fail(SAT_ERR_INVALID, "n_img*num_samples %lld outside [1, %d]", (long long)n_img * num_samples, h->max_rows);
+    if (T < 1) return fail(SAT_ERR_INVALID, "T must be >= 1");
+    if (num_samples > 4) return fail(SAT_ERR_UNSUPPORTED, "num_samples %d > 4 (draw more with further seeds)", num_samples);
+    RET(require_ready(h));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!h->smp) {
+        if (stream_capturing(st)) return fail(SAT_ERR_STATE, "sat_sample_loop_filtered: allocation during graph capture");
+        RET(dmalloc(&h->smp, 1));
+    }
+    // the filters live in device memory beside seed and temperature: a captured graph replays with any of them
+    CK(sample_params_launch(h->smp, seed, 1.0f / temperature, st, top_k, top_p));
+    h->launches += 1;
+    const int B = n_img * num_samples;
+    std::vector<long long> key = {6, (long long)contexts, n_img, num_samples, T, (long long)tokens, (long long)word_probs};
+    const int rc = run_graphed(h, key, st, [&]() -> int {
+        return loop_enqueue(h, contexts, B, T, nullptr, tokens, nullptr, nullptr, word_probs, st, num_samples, h->smp, true);
     });
     note_projected(h, rc == SAT_OK ? contexts : nullptr, n_img);   // (see sat_decode_loop)
     return rc;

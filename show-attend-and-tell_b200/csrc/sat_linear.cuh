@@ -230,10 +230,13 @@ __host__ __device__ inline DropGen drop_gen(unsigned long long seed, unsigned lo
 // (seed, row, step) is mixed once per row by two rounds of splitmix64 into a 64-bit key; each word then costs one
 // keyed 32-bit hash (lowbias32 with the key's halves entering before the first and between the two multiplies, a
 // bijection of the word for a given key).  sat_sample_uniform is this function on the host.
+// top_k / top_p are the filters of sat_sample_loop_filtered (0 / 1: off), read only by the filtered per-row kernel.
 struct SampleParams {
     unsigned long long seed;
     float inv_tau;          // 1 / temperature
     float pad;
+    int top_k;              // draw among the top_k most probable words (0 or >= V: all)
+    float top_p;            // ... and among the smallest prefix of those whose probability mass reaches top_p (1: all)
 };
 struct SampleKey {
     uint32_t k0, k1;

@@ -203,10 +203,247 @@ __global__ void __launch_bounds__(kRowThreads) rows_softmax_kernel(const RowsPar
     }
 }
 
+// ------------------------------------------------------------ filtered sampling (top-k / nucleus)
+// Words rank by (logit desc, index asc), the order of better().  Selection runs on order-preserving uint32 keys of the
+// raw logits (a larger float has a larger key; -0 is keyed as +0, so equal logits have equal keys) in three radix
+// digits of 11, 11 and 10 bits, with one 2048-bin histogram in shared memory.
+constexpr int kFiltBins = 2048;
+constexpr int kFiltBinsPerThread = kFiltBins / kRowThreads;
+
+__device__ __forceinline__ uint32_t filt_key(float v) {
+    const uint32_t u = __float_as_uint(v == 0.f ? 0.f : v);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float filt_unkey(uint32_t k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+// a word's nucleus mass: exp((x - max) / temperature) in 32.32 fixed point (at most 2^32 per word, so sums over any
+// V < 2^32 fit in 64 bits).  Integer sums are exact, hence independent of the order of the atomics.  NaN weighs 0.
+__device__ __forceinline__ unsigned long long filt_mass(float v, float mx, float itau) {
+    const float e = expf((v - mx) * itau);
+    return e > 0.f ? __float2ull_rz(e * 4294967296.0f) : 0ull;
+}
+
+// Radix descent.  weight(i, v, key) is the weight of word i (0: not a candidate).  Returns the key b of the word at which
+// the running weight, taken in key-descending order, first reaches `need` (weights of equal keys taken together); in
+// *left the weight still needed among the words of key b, in *eq their total weight.  frac >= 0: need = max(1,
+// ceil(frac * total weight)), fixed after the first digit (a total of 0 returns at once with *left = 0).  Otherwise
+// need must lie in [1, total weight].
+template <bool CACHED, typename W>
+__device__ uint32_t filt_descend(const float* x, const float* row_s, int V, unsigned long long need, double frac,
+                                 W weight, unsigned long long* hist, unsigned long long* sm_u,
+                                 unsigned long long* left, unsigned long long* eq) {
+    __shared__ uint32_t s_bin;
+    __shared__ unsigned long long s_left, s_eq;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    uint32_t prefix = 0;
+#pragma unroll 1
+    for (int pass = 0; pass < 3; ++pass) {
+        const int shift = pass == 0 ? 21 : (pass == 1 ? 10 : 0);
+        const uint32_t hi_mask = pass == 0 ? 0u : (pass == 1 ? 0xffe00000u : 0xfffffc00u);
+        const uint32_t dmask = pass == 2 ? 0x3ffu : 0x7ffu;
+#pragma unroll
+        for (int j = 0; j < kFiltBinsPerThread; ++j) hist[tid * kFiltBinsPerThread + j] = 0ull;
+        __syncthreads();
+        // (every thread has read the previous digit's result by now; the boundary bin is written after two barriers)
+        if (tid == 0) { s_bin = 0; s_left = 1; s_eq = 0; }
+#pragma unroll 1
+        for (int i = tid; i < V; i += kRowThreads) {
+            const float v = CACHED ? row_s[i] : x[i];
+            const uint32_t key = filt_key(v);
+            if ((key & hi_mask) != prefix) continue;
+            const unsigned long long w = weight(i, v, key);
+            if (w) atomicAdd(&hist[(key >> shift) & dmask], w);
+        }
+        __syncthreads();
+        // thread t owns bins [8t, 8t + 8): the weight above its bins is a suffix sum over the threads after it
+        unsigned long long own = 0;
+#pragma unroll
+        for (int j = 0; j < kFiltBinsPerThread; ++j) own += hist[tid * kFiltBinsPerThread + j];
+        unsigned long long suf = own;   // inclusive suffix sum inside the warp
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long y = __shfl_down_sync(0xffffffffu, suf, o);
+            if (lane + o < 32) suf += y;
+        }
+        if (lane == 0) sm_u[warp] = suf;
+        __syncthreads();
+        unsigned long long above = suf - own, total = 0;
+        for (int w = 0; w < kRowThreads / 32; ++w) {
+            total += sm_u[w];
+            if (w > warp) above += sm_u[w];
+        }
+        if (pass == 0 && frac >= 0.0) {
+            if (total == 0) {   // (uniform: every thread summed the same warp totals)
+                *left = *eq = 0ull;
+                return 0u;
+            }
+            const double c = ceil(frac * (double)total);
+            need = c < 1.0 ? 1ull : (c >= (double)total ? total : (unsigned long long)c);
+        }
+        if (above < need && need <= above + own) {
+#pragma unroll 1
+            for (int j = kFiltBinsPerThread - 1; j >= 0; --j) {
+                const unsigned long long hb = hist[tid * kFiltBinsPerThread + j];
+                if (need <= above + hb) {
+                    s_bin = tid * kFiltBinsPerThread + j;
+                    s_left = need - above;
+                    s_eq = hb;
+                    break;
+                }
+                above += hb;
+            }
+        }
+        __syncthreads();
+        prefix |= s_bin << shift;
+        need = s_left;
+    }
+    *left = need;
+    *eq = s_eq;
+    return prefix;
+}
+
+// Index of the c-th word (1 <= c, in index order) with key k that `cand` admits: a block prefix count over chunks of
+// kRowThreads consecutive words, stopping at the chunk that holds it.
+template <bool CACHED, typename C>
+__device__ int filt_nth(const float* x, const float* row_s, int V, uint32_t k, unsigned long long c, C cand,
+                        int* sm_cnt) {
+    __shared__ int s_idx;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) s_idx = V - 1;
+    unsigned long long base = 0;
+#pragma unroll 1
+    for (int i0 = 0; i0 < V; i0 += kRowThreads) {
+        const int i = i0 + tid;
+        const bool f = i < V && filt_key(CACHED ? row_s[i] : x[i]) == k && cand(i);
+        const unsigned bal = __ballot_sync(0xffffffffu, f);
+        if (lane == 0) sm_cnt[warp] = __popc(bal);
+        __syncthreads();
+        int off = 0, tot = 0;
+        for (int w = 0; w < kRowThreads / 32; ++w) {
+            if (w < warp) off += sm_cnt[w];
+            tot += sm_cnt[w];
+        }
+        if (f && base + off + __popc(bal & ((1u << lane) - 1u)) + 1 == c) s_idx = i;
+        base += tot;
+        __syncthreads();
+        if (base >= c) break;
+    }
+    return s_idx;
+}
+
+// Filtered sampling: one block per row.  Word i is kept when it is among the top_k words of the row (ties at the
+// boundary to the lower index) and inside the shortest prefix of those, in rank order, whose softmax(logits /
+// temperature) mass renormalised over them reaches top_p.  The draw is the Gumbel arg-max of the SMP instance over the
+// kept words, so a word that the unfiltered draw of the same (seed, row, step) picks is picked here when it is kept;
+// word_probs stay softmax(logits)[word] at temperature 1 over the whole row.
+template <bool CACHED>
+__global__ void __launch_bounds__(kRowThreads) rows_filter_kernel(const RowsParams p) {
+    extern __shared__ __align__(16) float row_s[];
+    __shared__ unsigned long long hist[kFiltBins];
+    __shared__ unsigned long long sm_u[kRowThreads / 32];
+    __shared__ ValIdx sm_vi[kRowThreads / 32];
+    __shared__ float sm_f[kRowThreads / 32];
+    __shared__ int sm_cnt[kRowThreads / 32];
+    if (threadIdx.x == 0) tl_begin(p.tl);
+    const int row = blockIdx.x;
+    const float* x = p.logits + (size_t)row * p.V;
+    const int V = p.V, n4 = V >> 2;
+    const SampleParams* sp = p.sample;
+    const float itau = sp->inv_tau;
+    const int top_k = sp->top_k;
+    const float top_p = sp->top_p;
+
+    float mr = -INFINITY;
+    if (CACHED) {
+        const float4* x4 = reinterpret_cast<const float4*>(x);
+        float4* d4 = reinterpret_cast<float4*>(row_s);
+#pragma unroll 1
+        for (int i4 = threadIdx.x; i4 < n4; i4 += kRowThreads) {
+            const float4 v = x4[i4];
+            d4[i4] = v;
+            mr = fmaxf(fmaxf(mr, v.x), fmaxf(v.y, fmaxf(v.z, v.w)));
+        }
+    } else {
+#pragma unroll 1
+        for (int i = threadIdx.x; i < V; i += kRowThreads) mr = fmaxf(mr, x[i]);
+    }
+    const float m = block_best(ValIdx{mr, 0}, sm_vi).v;   // (its barriers also publish row_s)
+
+    // top-k: kept when key > kk, or key == kk and i <= ki
+    uint32_t kk = 0u;
+    int ki = 0x7fffffff;
+    if (top_k > 0 && top_k < V) {
+        unsigned long long left, eq;
+        kk = filt_descend<CACHED>(x, row_s, V, (unsigned long long)top_k, -1.0,
+                                  [](int, float, uint32_t) { return 1ull; }, hist, sm_u, &left, &eq);
+        if (left < eq) ki = filt_nth<CACHED>(x, row_s, V, kk, left, [](int) { return true; }, sm_cnt);
+    }
+    auto in_k = [&](int i, uint32_t key) { return key > kk || (key == kk && i <= ki); };
+
+    // nucleus over the top-k words: kept when also key > pk, or key == pk and i <= pi
+    uint32_t pk = 0u;
+    int pi = 0x7fffffff;
+    if (top_p < 1.0f) {
+        const auto mass = [&](int i, float v, uint32_t key) { return in_k(i, key) ? filt_mass(v, m, itau) : 0ull; };
+        unsigned long long left, eq;
+        const uint32_t b = filt_descend<CACHED>(x, row_s, V, 0ull, (double)top_p, mass, hist, sm_u, &left, &eq);
+        if (left > 0) {   // (a row whose words all weigh 0, e.g. all -inf, keeps the top-k words)
+            pk = b;
+            // words of equal key weigh the same: the first ceil(left / w) of them in index order are kept
+            const unsigned long long w = filt_mass(filt_unkey(pk), m, itau);
+            const unsigned long long c = w ? (left + w - 1) / w : 1ull;
+            if (c * w < eq)
+                pi = filt_nth<CACHED>(x, row_s, V, pk, c, [&](int i) { return in_k(i, pk); }, sm_cnt);
+        }
+    }
+
+    const SampleKey sk = sample_key(sp->seed, row, p.step);
+    ValIdx best = {-INFINITY, 0x7fffffff};
+#pragma unroll 1
+    for (int i = threadIdx.x; i < V; i += kRowThreads) {
+        const float v = CACHED ? row_s[i] : x[i];
+        const uint32_t key = filt_key(v);
+        if (!in_k(i, key) || !(key > pk || (key == pk && i <= pi))) continue;
+        const float g = fmaf(v, itau, sample_gumbel(sample_bits(sk, i)));
+        if (better(g, i, best.v, best.i)) { best.v = g; best.i = i; }
+    }
+    best = block_best(best, sm_vi);
+    if (threadIdx.x == 0) {
+        if (p.tokens) p.tokens[(size_t)row * p.tokens_ld + p.step] = best.i;
+        if (p.next_word) p.next_word[row] = best.i;
+    }
+    if (p.word_probs) {
+        float s = 0.f;
+#pragma unroll 1
+        for (int i = threadIdx.x; i < V; i += kRowThreads) s += expf((CACHED ? row_s[i] : x[i]) - m);
+        s = block_sum(s, sm_f);
+        if (threadIdx.x == 0)   // (a row of NaN logits picks no word: probability 0, no read past the row)
+            p.word_probs[(size_t)row * p.tokens_ld + p.step] = (best.i >= 0 && best.i < V) ? expf(x[best.i] - m) / s : 0.f;
+    }
+    if (threadIdx.x == 0) tl_end(p.tl);
+}
+
 cudaError_t rows_softmax_launch(const RowsParams& p, int rows, cudaStream_t st) {
     if (p.topk > kMaxTopK) return cudaErrorInvalidValue;
     const size_t bytes = (size_t)p.V * sizeof(float);
     const bool cached = (p.V % 4) == 0 && bytes <= 96 * 1024 && (reinterpret_cast<uintptr_t>(p.logits) % 16) == 0;
+    if (p.sample && p.filter) {
+        if (p.forced || p.topk || p.probs || p.argmax || p.V < 2) return cudaErrorInvalidValue;
+        if (cached) {
+            static bool filt_attr_set = false;
+            if (!filt_attr_set) {
+                cudaError_t e = cudaFuncSetAttribute(rows_filter_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                     96 * 1024);
+                if (e != cudaSuccess) return e;
+                filt_attr_set = true;
+            }
+            rows_filter_kernel<true><<<rows, kRowThreads, bytes, st>>>(p);
+        } else {
+            rows_filter_kernel<false><<<rows, kRowThreads, 0, st>>>(p);
+        }
+        return cudaGetLastError();
+    }
     if (p.sample) {
         if (p.forced || p.topk || p.probs || p.argmax) return cudaErrorInvalidValue;
         if (cached) {
@@ -479,14 +716,17 @@ cudaError_t beam_maps_launch(const BeamParams& p, cudaStream_t st) {
 size_t beam_citem_bytes() { return sizeof(CItem); }
 
 // ---------------------------------------------------------------- sampling loop
-__global__ void sample_params_kernel(SampleParams* dst, unsigned long long seed, float inv_tau) {
+__global__ void sample_params_kernel(SampleParams* dst, unsigned long long seed, float inv_tau, int top_k, float top_p) {
     dst->seed = seed;
     dst->inv_tau = inv_tau;
     dst->pad = 0.f;
+    dst->top_k = top_k;
+    dst->top_p = top_p;
 }
 
-cudaError_t sample_params_launch(SampleParams* dst, unsigned long long seed, float inv_tau, cudaStream_t st) {
-    sample_params_kernel<<<1, 1, 0, st>>>(dst, seed, inv_tau);
+cudaError_t sample_params_launch(SampleParams* dst, unsigned long long seed, float inv_tau, cudaStream_t st, int top_k,
+                                 float top_p) {
+    sample_params_kernel<<<1, 1, 0, st>>>(dst, seed, inv_tau, top_k, top_p);
     return cudaGetLastError();
 }
 

@@ -29,6 +29,8 @@ struct RowsParams {
     const SampleParams* sample;   // sampling loop (no forced words, no top-k): the word is the arg-max of
                                   // logit / temperature + the Gumbel noise of (seed, row, step, word), as in the fused
                                   // vocabulary layer; word_probs stay softmax(logits) at temperature 1
+    int filter;           // with `sample`: draw only among the words kept by sample->top_k / top_p (filtered instance)
+    unsigned long long* tl;   // optional timeline cells of the filtered instance (debug option "trace" = 3)
 };
 
 struct PItem;
@@ -72,8 +74,10 @@ cudaError_t beam_update_launch(const BeamParams& p, cudaStream_t st);
 cudaError_t beam_finalize_launch(const BeamParams& p, cudaStream_t st);
 cudaError_t beam_maps_launch(const BeamParams& p, cudaStream_t st);   // after finalize, when res_alpha / res_probs
 size_t beam_citem_bytes();
-// sampling loop: *dst = {seed, inv_tau} (one thread, queued on the caller's stream ahead of a replayed graph)
-cudaError_t sample_params_launch(SampleParams* dst, unsigned long long seed, float inv_tau, cudaStream_t st);
+// sampling loop: *dst = {seed, inv_tau, top_k, top_p} (one thread, queued on the caller's stream ahead of a replayed
+// graph)
+cudaError_t sample_params_launch(SampleParams* dst, unsigned long long seed, float inv_tau, cudaStream_t st,
+                                 int top_k = 0, float top_p = 1.0f);
 // rows [r] of c_dst / h_dst = rows [r / G] of c_src / h_src ([rows / G, H] -> [rows, H], H % 4 == 0)
 cudaError_t bcast_state_launch(const float* c_src, const float* h_src, float* c_dst, float* h_dst, int rows, int G, int H,
                                cudaStream_t st);

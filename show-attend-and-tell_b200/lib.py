@@ -52,6 +52,7 @@ SIGNATURES = {
     "sat_decode_loop_maps": (C.c_int, [_P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
     "sat_beam_search_maps": (C.c_int, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
     "sat_sample_loop": (C.c_int, [_P, _P, _I, _I, _I, C.c_float, C.c_uint64, _P, _P, _P]),
+    "sat_sample_loop_filtered": (C.c_int, [_P, _P, _I, _I, _I, C.c_float, _I, C.c_float, C.c_uint64, _P, _P, _P]),
     "sat_sample_uniform": (C.c_double, [C.c_uint64, _L, _I, _I]),
     "sat_decode_step_host": (C.c_int, [_P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _P]),
     "sat_decode_loop_host": (C.c_int, [_P, _P, _I, _I, _P, _P, _P]),

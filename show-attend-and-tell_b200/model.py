@@ -687,16 +687,21 @@ class CaptionGenerator(object):
     # rows of one image per sat_sample_loop call (the attention kernels share an image's contexts between at most 4)
     SAMPLE_GROUP = 4
 
-    def sample_device(self, contexts, num_samples, num_steps, temperature=1.0, seed=None, want_word_probs=True):
+    def sample_device(self, contexts, num_samples, num_steps, temperature=1.0, seed=None, want_word_probs=True,
+                      top_k=0, top_p=1.0):
         """sat_sample_loop: num_samples captions per image drawn from softmax(logits / temperature).  contexts: CUDA
         tensor [n, L, D].  Returns tokens [n, K, T] int32 and word_probs [n, K, T] (softmax(logits)[word] at
         temperature 1) or None (persistent buffers, overwritten by the next call of the same kind).
         More than SAMPLE_GROUP samples are drawn in groups of SAMPLE_GROUP per image: group c (samples 4c .. 4c+3) is
-        a library call with seed + c * 0x9E3779B97F4A7C15 (mod 2^64), so group 0 is what a call with K <= 4 draws."""
+        a library call with seed + c * 0x9E3779B97F4A7C15 (mod 2^64), so group 0 is what a call with K <= 4 draws.
+        top_k (0: off) / top_p (1: off): draw only among the top_k most probable words, and among the smallest set of
+        those whose probability mass reaches top_p (sat_sample_loop_filtered); word_probs keep their meaning."""
         torch = self.torch
         n, K, T = contexts.shape[0], int(num_samples), int(num_steps)
         if K < 1:
             raise ValueError("num_samples must be >= 1")
+        top_k, top_p = int(top_k), float(top_p)
+        filtered = top_k != 0 or top_p != 1.0
         seed = self._sample_seed(seed)
         G = self.SAMPLE_GROUP
         parts = []
@@ -706,8 +711,13 @@ class CaptionGenerator(object):
             tokens = self._buf("s_tokens%d" % c, (n, kc, T), torch.int32)
             wprobs = self._buf("s_word_probs%d" % c, (n, kc, T), torch.float32) if want_word_probs else None
             sc = (seed + c * 0x9E3779B97F4A7C15) & 0xFFFFFFFFFFFFFFFF
-            self._check(self.lib.sat_sample_loop(self._h, self._p(contexts), n, kc, T, float(temperature), sc,
-                                                 self._p(tokens), self._p(wprobs), self._st()))
+            if filtered:
+                self._check(self.lib.sat_sample_loop_filtered(self._h, self._p(contexts), n, kc, T, float(temperature),
+                                                              top_k, top_p, sc, self._p(tokens), self._p(wprobs),
+                                                              self._st()))
+            else:
+                self._check(self.lib.sat_sample_loop(self._h, self._p(contexts), n, kc, T, float(temperature), sc,
+                                                     self._p(tokens), self._p(wprobs), self._st()))
             parts.append((tokens, wprobs))
         if len(parts) > 1:   # (on our stream: the concatenation is ordered after every group)
             with torch.cuda.stream(self.stream):
@@ -719,17 +729,19 @@ class CaptionGenerator(object):
         self._keep["sample"] = (contexts, tokens, wprobs, parts)
         return tokens, wprobs
 
-    def sample(self, contexts, num_samples=1, temperature=1.0, seed=None, num_steps=None, eos_id=None):
+    def sample(self, contexts, num_samples=1, temperature=1.0, seed=None, num_steps=None, eos_id=None, top_k=0,
+               top_p=1.0):
         """Sampled captions: per image, num_samples CaptionData drawn word by word from softmax(logits / temperature).
         sentence: the words up to and including the first eos_id (default config.eos_id), or all num_steps words;
         complete: whether the caption reached eos_id; word_probs: the model's probability (temperature 1) of each of
         those words; score: their fp64 product (beam search's convention).  seed: a given seed reproduces the call bit
-        for bit; None draws the next seed of this instance.  contexts: numpy or torch."""
+        for bit; None draws the next seed of this instance.  top_k / top_p: see sample_device (0 / 1: off).
+        contexts: numpy or torch."""
         cfg = self.config
         T = int(num_steps or cfg.max_caption_length)
         eos = int(cfg.eos_id if eos_id is None else eos_id)
         ctx = self._dev(contexts, self.torch.float32)
-        tokens, wprobs = self.sample_device(ctx, num_samples, T, temperature, seed)
+        tokens, wprobs = self.sample_device(ctx, num_samples, T, temperature, seed, top_k=top_k, top_p=top_p)
         self.torch.cuda.synchronize(self.device)
         tokens, wprobs = tokens.cpu().numpy(), wprobs.cpu().numpy()
         results = []

@@ -9,10 +9,17 @@ At the workload-2 model shape of bench.py (L=196, D=512, H=1024, V=10000, T=20),
   (b) sample_64x1: sampling, 64 images x 1 caption, with word probabilities;
   (b') sample_64x1_noprobs: the same without them (the draw alone);
   (c) sample_16x4: sampling, 16 images x 4 captions (the 4 rows of an image share its contexts), with word probabilities;
-  (d) beam_16x4: beam search, 16 images x beam 4, for comparison.
+  (d) beam_16x4: beam search, 16 images x beam 4, for comparison;
+  (e) sample_64x1_topk50, sample_64x1_topp09, sample_16x4_topp09: filtered sampling (sat_sample_loop_filtered) with
+      top_k = 50 or top_p = 0.9, with word probabilities.  The vocabulary layer writes the logits and the filtered
+      per-row kernel draws, one step at a time.
+Then, in a block of its own (the option change drops the captured graphs), (f) sample_64x1_overlap0: plain sampling
+forced into that per-step layout (option "overlap" = 0).  So (f) - (b) is the cost of the layout and (e) - (f) that of
+writing the logits and running the filter kernel.
 So (b') - (a) is the cost of the Gumbel draw, (a') - (a) that of the softmax partials of the word probabilities.
-Then (unless --no-trace) one eager loop of (a), (a'), (b) and (b') with in-kernel timeline stamps (option "trace" = 3):
-the mean time from first CTA start to last CTA end of each kernel family per step.
+Then (unless --no-trace) one eager loop of (a), (a'), (b), (b'), (e) and (f) with in-kernel timeline stamps (option
+"trace" = 3): the mean time from first CTA start to last CTA end of each kernel family per step ("filter": the filtered
+per-row kernel).
 Prints one JSON line: the card's name and power limit, the median ms per call of each leg and the per-family times.
 """
 import argparse
@@ -89,30 +96,46 @@ def main():
         "sample_64x1_noprobs": lambda: m.sample_device(ctx, 1, T, 1.0, next(seeds), want_word_probs=False),
         "sample_16x4": lambda: m.sample_device(ctx16, 4, T, 1.0, next(seeds)),
         "beam_16x4": lambda: m.beam_device(ctx16, 4, T, 2),
+        "sample_64x1_topk50": lambda: m.sample_device(ctx, 1, T, 1.0, next(seeds), top_k=50),
+        "sample_64x1_topp09": lambda: m.sample_device(ctx, 1, T, 1.0, next(seeds), top_p=0.9),
+        "sample_16x4_topp09": lambda: m.sample_device(ctx16, 4, T, 1.0, next(seeds), top_p=0.9),
     }
-    for f in calls.values():
-        for _ in range(max(args.warmup, 3)):   # eager run, capture, replays
-            f()
-    torch.cuda.synchronize()
-    ms = {k: [] for k in calls}
     st = m.stream
-    for _ in range(args.rounds):
-        for k, f in calls.items():
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            with torch.cuda.stream(st):
-                e0.record(st)
-                for _ in range(args.steps):
-                    f()
-                e1.record(st)
-            torch.cuda.synchronize()
-            ms[k].append(e0.elapsed_time(e1) / args.steps)
+
+    def timed(legs):
+        for f in legs.values():
+            for _ in range(max(args.warmup, 3)):   # eager run, capture, replays
+                f()
+        torch.cuda.synchronize()
+        ms = {k: [] for k in legs}
+        for _ in range(args.rounds):
+            for k, f in legs.items():
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                with torch.cuda.stream(st):
+                    e0.record(st)
+                    for _ in range(args.steps):
+                        f()
+                    e1.record(st)
+                torch.cuda.synchronize()
+                ms[k].append(e0.elapsed_time(e1) / args.steps)
+        return ms
+
+    ms = timed(calls)
+    overlap0 = {"sample_64x1_overlap0": calls["sample_64x1"]}
+    m.set_option("overlap", 0)
+    ms.update(timed(overlap0))
+    m.set_option("overlap", 2)
     med = {k: sorted(v)[len(v) // 2] for k, v in ms.items()}
     out = {"metric": "sample_cost", "gpu": card, "shape": dict(L=L, D=D, H=H, V=V, T=T), "steps": args.steps,
            "rounds": args.rounds, "ms_per_call": med,
            "vs_greedy_pct": {k: 100.0 * (v / med["greedy"] - 1.0) for k, v in med.items()}, "ms_per_call_rounds": ms}
     if not args.no_trace:
         out["trace_us"] = {k: family_times(m, calls[k])
-                           for k in ("greedy", "greedy_probs", "sample_64x1", "sample_64x1_noprobs")}
+                           for k in ("greedy", "greedy_probs", "sample_64x1", "sample_64x1_noprobs",
+                                     "sample_64x1_topk50", "sample_64x1_topp09", "sample_16x4_topp09")}
+        m.set_option("overlap", 0)
+        out["trace_us"]["sample_64x1_overlap0"] = family_times(m, overlap0["sample_64x1_overlap0"])
+        m.set_option("overlap", 2)
     m.close()
     print(json.dumps(out), flush=True)
 
