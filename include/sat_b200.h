@@ -220,7 +220,10 @@ int sat_beam_search_host(sat_handle* h, const float* contexts_host, int32_t n_im
 
 /* individually callable kernels of one step (profiling / unit tests).  Rows = n_img * group;
  * `group` rows of one image share its contexts (beams).
- *   sat_attention_fwd : attend + context vector (model.py:262-264) given the state h [rows,H]
+ *   sat_attention_fwd : attend + context vector (model.py:262-264) given the state h [rows,H]: alpha [rows,L]
+ *                       (may be NULL) and context [rows,D].  With the 2-layer attend the projection of the contexts
+ *                       is cached by contexts pointer and n_img, as for sat_decode_step: after writing new values
+ *                       into the same contexts buffer, call sat_prepare_contexts again
  *   sat_lstm_fwd      : embedding lookup + LSTMCell (model.py:272-279)
  *   sat_vocab_gemm    : decode (model.py:282-287) -> logits [rows,V]                         */
 int sat_attention_fwd(sat_handle* h, const float* contexts, const float* output, float* alpha, float* context,
