@@ -224,8 +224,11 @@ int sat_beam_search_host(sat_handle* h, const float* contexts_host, int32_t n_im
  *                       (may be NULL) and context [rows,D].  With the 2-layer attend the projection of the contexts
  *                       is cached by contexts pointer and n_img, as for sat_decode_step: after writing new values
  *                       into the same contexts buffer, call sat_prepare_contexts again
- *   sat_lstm_fwd      : embedding lookup + LSTMCell (model.py:272-279)
- *   sat_vocab_gemm    : decode (model.py:282-287) -> logits [rows,V]                         */
+ *   sat_lstm_fwd      : embedding lookup + LSTMCell (model.py:272-279) on context [rows,D], last_word [rows],
+ *                       last_memory and last_output [rows,H]: writes memory (c) and output (h) [rows,H]
+ *   sat_vocab_gemm    : decode (model.py:282-287) of output [rows,H], context [rows,D] and last_word [rows]:
+ *                       writes logits [rows,V] and nothing else (no arg-max: words are chosen by the loops)
+ * Both gather embedding rows without a range check: every last_word must lie in [0, V).      */
 int sat_attention_fwd(sat_handle* h, const float* contexts, const float* output, float* alpha, float* context,
                       int32_t n_img, int32_t group, void* stream);
 int sat_lstm_fwd(sat_handle* h, const float* context, const int32_t* last_word, const float* last_memory,
