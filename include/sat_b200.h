@@ -304,6 +304,33 @@ int sat_train_forward_backward_grouped(sat_handle* h, const float* params, float
  * Needs no handle: runs on the current device.  SAT_ERR_INVALID for null tokens / masks, rows < 0 or T < 1. */
 int sat_caption_masks(const int32_t* tokens, int32_t rows, int32_t T, int32_t eos_id, float* masks,
                       double* mask_sum, void* stream);
+/* CIDEr-D (the semantics of coco-caption's cider_scorer.py and of the CiderD scorer of self-critical training) of
+ * word-id captions against their references: the reward of self-critical training and a validation metric.
+ * A row (candidate or reference) ends after its first eos_id (which counts as a word), or before its first id < 0
+ * (padding) or >= vocabulary_size.  For n = 1..4, v_n(c)[g] = count_c(g) * (log N - log max(1, df(g))) over the n-grams
+ * g of c; "length" = the number of bigrams (both reference scorers compute it so); per reference r,
+ * s_n = sum over distinct g of c of min(v_n(c)[g], v_n(r)[g]) * v_n(r)[g], divided by |v_n(c)| |v_n(r)| when both are
+ * non-zero, times exp(-(len(c) - len(r))^2 / 72); CIDEr-D = 10 * mean over the non-empty references of mean over n of
+ * s_n (0 for an image without one).  df(g) = number of corpus images whose references, taken together, contain g, and
+ * N = the corpus's number of images: self-critical training builds the table from the training references,
+ * coco-caption from the evaluated set's own references.
+ *
+ * sat_cider_create: the document-frequency table of a corpus refs_host [n_img, R, T_ref] int32 on the HOST (an
+ * all-padding row is no reference), built on the host and uploaded to the device current at the call (a table of
+ * about 12 bytes x 2 x the corpus's distinct n-grams).  SAT_ERR_INVALID for n_img < 1, R < 1, T_ref < 1 or
+ * vocabulary_size outside [2, 65535] (an n-gram key holds four 16-bit word ids).
+ * sat_cider_d: scores [n_img, C] (device float) = CIDEr-D of candidates [n_img, C, T] against refs [n_img, R, T_ref]
+ * (device int32), with the eos_id, vocabulary_size and table of `c`.  One CTA per image: the references' n-gram
+ * weights are formed once and shared by the C candidates.  fp64 arithmetic in a fixed summation order: the result is
+ * bit-reproducible.  Asynchronous on `stream`.  Limits: R <= 8, T <= 64, T_ref <= 64 (SAT_ERR_UNSUPPORTED beyond);
+ * SAT_ERR_INVALID for null pointers, n_img < 0 or C, T, R, T_ref < 1.  Nothing is enqueued on an error. */
+typedef struct sat_cider sat_cider;
+int sat_cider_create(const int32_t* refs_host, int64_t n_img, int32_t R, int32_t T_ref, int32_t eos_id,
+                     int32_t vocabulary_size, sat_cider** out);
+void sat_cider_destroy(sat_cider* c);
+int sat_cider_d(const sat_cider* c, const int32_t* candidates, int32_t n_img, int32_t C, int32_t T,
+                const int32_t* refs, int32_t R, int32_t T_ref, float* scores, void* stream);
+
 /* adds the L2-regulariser gradient, clips by the global norm (clip_gradients, config.py:36) and applies TF Adam
  * (config.py:32-43).  step counts from 1.  grad_norm (device, 1 float, may be NULL) receives the squared norm. */
 int sat_train_apply(sat_handle* h, float* params, float* grads, float* adam_m, float* adam_v, int64_t step, float lr,

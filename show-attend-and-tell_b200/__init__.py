@@ -10,6 +10,7 @@ from .config import Config  # noqa: F401
 from .lib import SatError, load_library, library_path  # noqa: F401
 from .model import CaptionGenerator, weight_shapes  # noqa: F401
 from .captions import Vocabulary, assemble_captions, write_eval_results, write_test_results  # noqa: F401
+from .cider import CiderD  # noqa: F401
 
 __all__ = ["Config", "CaptionGenerator", "SatError", "load_library", "library_path", "weight_shapes", "Vocabulary",
-           "assemble_captions", "write_eval_results", "write_test_results"]
+           "assemble_captions", "write_eval_results", "write_test_results", "CiderD"]

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libsat_b200.so")
 STAMP = os.path.join(HERE, "build", "stamp.txt")
-SOURCES = ["sat_api.cu", "sat_linear.cu", "sat_chain.cu", "sat_attention.cu", "sat_rows.cu", "sat_train.cu"]
+SOURCES = ["sat_api.cu", "sat_linear.cu", "sat_chain.cu", "sat_attention.cu", "sat_rows.cu", "sat_train.cu", "sat_cider.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3", "--expt-relaxed-constexpr",

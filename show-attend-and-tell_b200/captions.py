@@ -149,3 +149,18 @@ def scst_advantages(rewards, num_samples, baseline="greedy"):
     else:
         raise ValueError("baseline must be 'greedy' or 'mean', got %r" % (baseline,))
     return samples - base, float(samples.mean()), float(base.mean())
+
+
+def scst_advantages_torch(rewards, num_samples, baseline="greedy"):
+    """scst_advantages with torch ops on a rewards tensor (e.g. CIDEr-D scores on the device), in float64 like it and
+    without reading anything back: (advantages [n, K] float64, mean sample reward, mean baseline reward), the two
+    means as 0-dim tensors on the rewards' device.  The caller has validated baseline and K."""
+    K = int(num_samples)
+    r = rewards.double()
+    if baseline == "greedy":
+        samples = r[:, :K]
+        base = r[:, K:K + 1].expand(-1, K)
+    else:
+        samples = r
+        base = (r.sum(dim=1, keepdim=True) - r) / (K - 1)
+    return samples - base, samples.mean(), base.mean()

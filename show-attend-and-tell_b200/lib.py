@@ -73,6 +73,9 @@ SIGNATURES = {
     "sat_train_init_grouped": (C.c_int, [_P, _I, _I, _I, C.c_float, C.c_float, C.c_float, C.c_float]),
     "sat_train_forward_backward_grouped": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _I, C.c_uint64, _P, _I, _P, _P]),
     "sat_caption_masks": (C.c_int, [_P, _I, _I, _I, _P, _P, _P]),
+    "sat_cider_create": (C.c_int, [_P, _L, _I, _I, _I, _I, C.POINTER(_P)]),
+    "sat_cider_destroy": (None, [_P]),
+    "sat_cider_d": (C.c_int, [_P, _P, _I, _I, _I, _P, _I, _I, _P, _P]),
     "sat_train_apply": (C.c_int, [_P, _P, _P, _P, _P, _L, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, _P,
                                   _P]),
     "sat_train_apply_opt": (C.c_int, [_P, _P, _P, _P, _P, _P, _L, C.POINTER(Optimizer), _P, _P]),

@@ -477,7 +477,7 @@ class CaptionGenerator(object):
         return fb(self._step_seed(seed), None, B)
 
     def scst_step(self, contexts, reward_fn, num_samples=5, baseline="greedy", temperature=1.0, seed=None,
-                  sample_seed=None, sync=True):
+                  sample_seed=None, sync=True, references=None):
         """One self-critical (SCST) policy-gradient step on a shard of images.
 
           1. the decode weights are refreshed from the training parameters (no host synchronisation);
@@ -496,9 +496,19 @@ class CaptionGenerator(object):
         Needs train_setup(n_img, group=num_samples).  With torch.distributed initialised, the mask sum of the whole
         batch and the gradient sum travel in train_step's single collective.  Returns the losses, the mean sample
         reward, the mean baseline reward and the gradient norm (sync=False: the losses [4] and the squared gradient
-        norm [1] as device tensors, the rewards as floats)."""
-        from .captions import cut_after_eos, scst_advantages
+        norm [1] as device tensors, the rewards as floats).
+        Built-in reward: reward_fn = a CiderD instance and references = this batch's reference captions [n, R, T_ref]
+        (device or host, -1 padded; R <= 8, T_ref <= 64).  Steps 4-5 then run on the device, in stream order: the K
+        samples and the greedy caption of each image are scored by sat_cider_d, and the advantages follow from the
+        scores in float64 (captions.scst_advantages_torch) into the row weights.  Nothing waits for the host, so with
+        sync=False the call returns once the step is queued, and the sample and baseline rewards are 0-dim float64
+        device tensors instead of floats."""
+        from .captions import cut_after_eos, scst_advantages, scst_advantages_torch
+        from .cider import CiderD
         torch = self.torch
+        device_reward = isinstance(reward_fn, CiderD)
+        if device_reward and references is None:
+            raise ValueError("scst_step with a CiderD reward needs this batch's references [n, R, T_ref]")
         cfg = self.config
         K = int(num_samples)
         if baseline not in ("greedy", "mean"):
@@ -521,14 +531,22 @@ class CaptionGenerator(object):
         with torch.cuda.stream(self.stream):
             sent.copy_(tokens.reshape(B, T))
         greedy = self.loop_device(ctx, T)[0] if baseline == "greedy" else None
-        self.stream.synchronize()
-        toks = sent.cpu().numpy().reshape(n, K, T)
-        gt = greedy.cpu().numpy() if greedy is not None else None
-        caps = [[cut_after_eos(toks[i, k], eos) for k in range(K)] + ([cut_after_eos(gt[i], eos)] if gt is not None else [])
-                for i in range(n)]
-        adv, r_sample, r_base = scst_advantages(reward_fn(caps), K, baseline)
         w = self._buf("scst_w", (B,), torch.float32)
-        w.copy_(torch.from_numpy(np.ascontiguousarray(adv.reshape(-1), dtype=np.float32)))
+        if device_reward:
+            with torch.cuda.stream(self.stream):
+                cand = tokens if greedy is None else torch.cat([tokens, greedy[:, None, :]], 1)
+            rewards = reward_fn.scores(cand, references, stream=self.stream)
+            with torch.cuda.stream(self.stream):
+                adv, r_sample, r_base = scst_advantages_torch(rewards, K, baseline)
+                w.copy_(adv.reshape(-1))
+        else:
+            self.stream.synchronize()
+            toks = sent.cpu().numpy().reshape(n, K, T)
+            gt = greedy.cpu().numpy() if greedy is not None else None
+            caps = [[cut_after_eos(toks[i, k], eos) for k in range(K)] + ([cut_after_eos(gt[i], eos)] if gt is not None else [])
+                    for i in range(n)]
+            adv, r_sample, r_base = scst_advantages(reward_fn(caps), K, baseline)
+            w.copy_(torch.from_numpy(np.ascontiguousarray(adv.reshape(-1), dtype=np.float32)))
         mk = self._buf("scst_masks", (B, T), torch.float32)
         msum = self._buf("scst_msum", (1,), torch.float64)
         self._sync_in()
@@ -544,7 +562,7 @@ class CaptionGenerator(object):
             return dict(losses=losses, gradient_norm2=norm2, sample_reward=r_sample, baseline_reward=r_base)
         ce, acc, att, reg = [float(x) for x in losses.tolist()]
         return dict(cross_entropy_loss=ce, accuracy=acc, attention_loss=att, reg_loss=reg, total_loss=ce + att + reg,
-                    sample_reward=r_sample, baseline_reward=r_base, gradient_norm=float(norm2.item()) ** 0.5,
+                    sample_reward=float(r_sample), baseline_reward=float(r_base), gradient_norm=float(norm2.item()) ** 0.5,
                     global_step=self.global_step)
 
     def train_step(self, contexts, sentences, masks, seed=None, sync=True, next_masks=None):
