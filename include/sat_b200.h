@@ -256,7 +256,10 @@ int sat_dense_fwd(sat_handle* h, const float* x, const float* w_tf, const float*
  * the attend/fc_1a products on the caller's stream (default: a second, low-priority stream of the library's own; 2 / 3:
  * only the forward / only the backward ones);
  * SAT_TRAIN_FUSE_SOFTMAX=0 / 2 un-fuses the softmax kernels (both directions / the backward one only); SAT_TRAIN_FUSE_PACK=0
- * packs the operands of the batch-row products in launches of their own instead of in their producer kernels.
+ * packs the operands of the batch-row products in launches of their own instead of in their producer kernels;
+ * SAT_TRAIN_ATTBWD_WAVE=1 runs the attention scorer's backward as one resident wave (a 64-register build of the kernel).
+ * params, grads and contexts must be 16-byte aligned (the step reads them with vector loads); every entry point below
+ * returns SAT_ERR_INVALID, with nothing enqueued, for a buffer that is not.
  * Word ids outside [0, vocabulary_size) read as zero rows, contribute no gradient and are counted
  * (sat_get_info "train_bad_ids"). */
 int sat_train_init(sat_handle* h, int32_t B, int32_t T, float fc_drop_rate, float lstm_drop_rate,

@@ -2030,6 +2030,10 @@ static int train_forward_backward(sat_handle* h, const float* params, float* gra
                                   int32_t global_batch, float* losses, void* stream) {
     if (!h || !params || !grads || !contexts || !sentences || !masks || !losses)
         return sat_fail(SAT_ERR_INVALID, "sat_train_forward_backward: null argument");
+    // the packing kernels read W^T of the batch-row layers (params) and the contexts as float4, the fused scorer the
+    // gradient rows (grads): a buffer off by a few floats is refused here, not met as a misaligned load on the device
+    if (((reinterpret_cast<uintptr_t>(params) | reinterpret_cast<uintptr_t>(grads) | reinterpret_cast<uintptr_t>(contexts)) & 15) != 0)
+        return sat_fail(SAT_ERR_INVALID, "sat_train_forward_backward: params, grads and contexts must be 16-byte aligned");
     TrainState* s = (TrainState*)*sat_handle_train_slot(h);
     const int32_t B = n_img * group;
     if (!s || s->n_img * s->group != B || s->T != T) return sat_fail(SAT_ERR_STATE, "call sat_train_init(B=%d, T=%d) first", B, T);
