@@ -170,6 +170,7 @@ struct sat_handle {
     int trace_at = 0;      // with trace == 1: index of the dense launch (counted from the option call) to stamp
     bool lin_w_dynamic = false;   // next dense launch: its weight operand comes from the preceding kernel
     int att_loop_grid = 0; // CTAs of the last attention launch that ran beside the vocabulary layer (decode loop)
+    int att_loop_beside = 0; // 1: that launch ran beside its predecessor (did not wait for it before streaming)
     int tl_count = 0;      // with trace == 3: launches recorded so far ({min start, max end} per launch)
     std::vector<std::string> tl_names;
 
@@ -502,6 +503,7 @@ extern "C" int sat_get_info(sat_handle* h, const char* key, int64_t* value) {
     else if (k == "trace_ptr") *value = (int64_t)(uintptr_t)h->trace;
     else if (k == "tl_count") *value = h->tl_count;
     else if (k == "att_loop_grid") *value = h->att_loop_grid;
+    else if (k == "att_loop_beside") *value = h->att_loop_beside;
     else if (k.rfind("tl_tag_", 0) == 0) {   // family code of timeline entry i: index into the tag list, grid in the high bits
         const int i = atoi(k.c_str() + 7);
         if (i < 0 || i >= (int)h->tl_names.size()) return fail(SAT_ERR_INVALID, "timeline index");
@@ -937,9 +939,11 @@ static int attention_impl(sat_handle* h, const float* ctx, int n_img, int G, con
     if (sm_budget <= 0 && h->opt_att_sms > 0) sm_budget = h->opt_att_sms;   // experiment knob
     if (!att_plan(ap, h->smem_optin, sm_budget > 0 ? sm_budget : h->num_sms))
         return fail(SAT_ERR_UNSUPPORTED, "attention shape unsupported (G=%d L=%d D=%d)", G, ap.L, ap.D);
-    if (nowait && (!ap.wpc || n_img > ap.grid)) {
-        // running beside the vocabulary layer on the SMs it leaves idle only pays when the kernel can skip the
-        // wait (warp-per-chunk kernel) and one CTA per image fits that budget; otherwise: whole GPU, in order
+    if (nowait && (!ap.wpc || (h->att_qflag && n_img > ap.grid))) {
+        // running beside the predecessor only works when the kernel can skip the wait (warp-per-chunk kernel).  On
+        // fewer SMs than images CTA row ranges cross image boundaries, which the decode loop's attention takes (on
+        // an H100 the vocabulary layer leaves 53 SMs for 64 images); the chained launch wants one CTA per image.
+        // Otherwise: whole GPU, in order
         nowait = false;
         ap.occ = h->opt_att_occ;
         ap.warps = h->opt_att_warps;
@@ -977,7 +981,10 @@ static int attention_impl(sat_handle* h, const float* ctx, int n_img, int G, con
         ap.qflag = h->att_qflag;
         ap.qtarget = h->att_qtarget;
     }
-    if (q_ready && !h->opt_att_reuse_q) h->att_loop_grid = ap.grid;
+    if (q_ready && !h->opt_att_reuse_q) {
+        h->att_loop_grid = ap.grid;
+        h->att_loop_beside = ap.nowait;
+    }
     ap.dbg = h->opt_trace == 2 ? h->trace : nullptr;
     ap.tl = nullptr;
     if (h->opt_trace == 3 && h->tl_count < 4000) {
@@ -1340,6 +1347,11 @@ static int loop_enqueue_overlap(sat_handle* h, const float* ctx, int B, int T, c
 // pdl_wait) and nothing from the vocabulary layer, so it starts on the SMs the vocabulary layer's one-wave
 // grid leaves idle and the two run side by side without a second stream; it only waits for its predecessor
 // right before it exits, which keeps "kernel k complete => kernel k-1 complete" for the LSTM that follows.
+// Its grid is the SMs left over (132 - 79 = 53 on an H100 at V = 10000), also when that is fewer than the images:
+// CTA row ranges then cross image boundaries.  It must stay the vocabulary layer's PDL successor on this stream:
+// the layer's fused arg-max meets at a grid-wide counter (am_ctr, sat_linear.cu) and so needs all its CTAs
+// resident at once; the attention only becomes launchable once every one of them has passed its pdl_wait, so it
+// can never take an SM one of them still needs.
 static int loop_enqueue_chain(sat_handle* h, const float* ctx, int B, int T, const int32_t* forced, int32_t* tokens,
                               float* logits_all, float* alphas, float* word_probs, cudaStream_t st, bool prepared = false,
                               int G = 1, const SampleParams* smp = nullptr) {
